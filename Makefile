@@ -1,6 +1,6 @@
-# Builds the product library kvazaar_b200/libkvzcuda.so (sm_100a only) and, via oracle/Makefile, the test oracles.
+# Builds the product library kvazaar_b200/libkvzcuda.so (H100, sm_90a only) and, via oracle/Makefile, the test oracles.
 NVCC      ?= nvcc
-ARCH      := -gencode arch=compute_100a,code=sm_100a
+ARCH      := -gencode arch=compute_90a,code=sm_90a
 # -fmad=false: cost arithmetic must not be contracted into FMAs (SURVEY.md H3); everything else is integer.
 NVFLAGS   := $(ARCH) -O3 -lineinfo -std=c++17 -fmad=false -Xcompiler -fPIC,-Wall -Iinclude
 SRCDIR    := kvazaar_b200/csrc

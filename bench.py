@@ -57,14 +57,14 @@ def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "fallback (H100 SXM data sheet, HBM3)"
 
 
 def config_of(wl):
     """identical for both arms: what is encoded, not how"""
     return {"workload": wl["name"], "resolution": f"{wl['w']}x{wl['h']}", "preset": wl["preset"], "qp": wl["qp"], "intra_period": 1,
             "bit_depth": 8, "clip": f"{DISTINCT} distinct synthetic pictures (tools/synth_yuv.py, seed 1234) cycled",
-            "l2": "every picture is read once; the pictures in flight (> 126 MB) exceed L2"}
+            "l2": "every picture is read once; the pictures in flight exceed the 50 MB L2"}
 
 
 def clip_path(wl):
@@ -106,9 +106,10 @@ def sha(path):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (one streaming nvidia-smi process, 100 ms period)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region (one streaming nvidia-smi process, 100 ms period), and
+    the card's name and power limit, which belong beside every number of the line."""
     Q = "clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown," \
-        "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
+        "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,name,power.limit"
 
     def __init__(self, index):
         self.index, self.proc, self.rows = index, None, []
@@ -133,7 +134,7 @@ class ClockSampler:
                 out = ""
             for ln in out.splitlines():
                 c = [x.strip() for x in ln.split(",")]
-                if len(c) >= 7:
+                if len(c) >= 9:
                     self.rows.append(c)
 
     def summary(self):
@@ -143,7 +144,8 @@ class ClockSampler:
         reasons = [name for i, name in enumerate(("hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"))
                    if any(r[3 + i] == "Active" for r in self.rows)]
         return {"sm_mhz": sm[len(sm) // 2], "sm_max_mhz": float(self.rows[0][1]), "reasons": reasons,
-                "power_w_max": max(float(r[2]) for r in self.rows), "samples": len(self.rows)}
+                "power_w_max": max(float(r[2]) for r in self.rows), "samples": len(self.rows), "gpu": self.rows[0][7],
+                "power_limit_w": float(self.rows[0][8])}
 
 
 # ------------------------------------------------------------------------------------------------ reference arm
@@ -201,8 +203,50 @@ def driver_config(wl):
     return c
 
 
+DUMP_SAMPLE = 1 << 22    # arrays longer than this are dumped as a fixed, seeded sample of this many elements
+
+
+CU_DTYPE = np.dtype([("type", "u1"), ("depth", "u1"), ("part_size", "u1"), ("tr_depth", "u1"), ("tr_skip", "u1"), ("qp", "u1"),
+                     ("mode", "i1"), ("mode_chroma", "i1"), ("cbf", "<u2"), ("pad", "<u2")])        # kvz_cuda_ctu_cu
+
+
+def fetch_result(res, w, h):
+    """Host copies of what kvz_cuda_ctu_wait_device handed back for one picture: CU records (one per 4x4 luma block),
+    coefficients, SAO parameters, final picture."""
+    import torch
+
+    def fetch(ptr, nbytes):
+        class Dev:  # a raw device pointer seen as a byte array (CUDA array interface, version 3)
+            __cuda_array_interface__ = {"shape": (nbytes,), "typestr": "|u1", "data": (ptr, False), "version": 3}
+        return torch.as_tensor(Dev(), device="cuda").cpu().numpy()
+
+    nctu = res.width_in_lcu * res.height_in_lcu
+    rows = res.height_in_lcu * 16
+    cu = fetch(res.cu, rows * res.cu_stride * CU_DTYPE.itemsize).view(CU_DTYPE).reshape(rows, res.cu_stride)
+    return {"cu": cu[:(h + 3) // 4, :(w + 3) // 4], "sao": fetch(res.sao, nctu * 2 * 17 * 4).view("<i4").reshape(nctu, 2, 17),
+            "coeff": fetch(res.coeff, nctu * 6144 * 2).view("<i2"), "rec": fetch(res.rec, w * h * 3 // 2)}
+
+
+def write_outputs(out_dir, out):
+    """DIR/<name>.npy: the CU fields as [rows, columns, field], the coefficients and the final picture (in full or, above
+    DUMP_SAMPLE elements, at a fixed seeded sample of positions, the same for every run) in float32, which holds these
+    8- and 16-bit values exactly; the SAO parameters (int32 fields, distortions among them) in float64."""
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "sao.npy"), out["sao"].astype(np.float64))
+    arrays = {"cu": np.stack([out["cu"][f] for f in CU_DTYPE.names if f != "pad"], axis=-1)}
+    for name in ("coeff", "rec"):
+        a = out[name]
+        if a.size > DUMP_SAMPLE:
+            a = a[np.sort(np.random.default_rng(1234).choice(a.size, DUMP_SAMPLE, replace=False))]
+        arrays[name] = a
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a.astype(np.float32))
+
+
 def device_leg(args, wl, local, frames_per_step, barrier):
-    """`value`: pictures resident in HBM through the driver alone; returns (seconds for K steps, launches, mean search-kernel ms)"""
+    """`value`: pictures resident in HBM through the driver alone; returns (seconds for K steps, launches, mean search-kernel ms).
+    With --dump-outputs, the slot of the last picture of the last timed step is held when that picture completes and its
+    results are copied out after the run: every timed picture is submitted before it, so the timed region is unchanged."""
     import torch
     import kvazaar_b200 as kb
     lib = C.CDLL(kb.LIB_PATH)
@@ -217,6 +261,8 @@ def device_leg(args, wl, local, frames_per_step, barrier):
     lib.kvz_cuda_last_error.restype = C.c_char_p
     cfg = driver_config(wl)
     slots = args.slots or (args.owf or wl["owf"]) + 1          # as many pictures in flight as the encoder keeps (owf + 1)
+    if args.dump_outputs and slots < 2:
+        raise SystemExit("bench.py: --dump-outputs holds one slot until the end of the run and needs at least 2 slots")
     enc = lib.kvz_cuda_ctu_open(C.byref(cfg), slots)
     if not enc:
         raise RuntimeError(f"kvz_cuda_ctu_open: {lib.kvz_cuda_last_error()}")
@@ -260,14 +306,17 @@ def device_leg(args, wl, local, frames_per_step, barrier):
                                                        cfg.lambda_, cfg.lambda_sqrt, wl["qp"])
                     if s < 0:
                         raise RuntimeError(f"submit: {lib.kvz_cuda_last_error()}")
-                    pending.append(s)
+                    pending.append((i, s))
                 if not pending:
                     return
-                s = pending.pop(0)
+                i, s = pending.pop(0)
                 if lib.kvz_cuda_ctu_wait_device(enc, s, C.byref(res)) != 0:
                     raise RuntimeError(f"wait: {lib.kvz_cuda_last_error()}")
                 ms = res.search_kernel_ms
-                lib.kvz_cuda_ctu_release(enc, s)
+                if args.dump_outputs and i == n_warm + n_timed - 1:
+                    state["dump"] = (s, DevResult.from_buffer_copy(res))          # released after the run
+                else:
+                    lib.kvz_cuda_ctu_release(enc, s)
                 with lock:
                     state["done"] += 1
                     done = state["done"]
@@ -290,6 +339,10 @@ def device_leg(args, wl, local, frames_per_step, barrier):
         t.join()
     if state["err"]:
         raise state["err"]
+    if args.dump_outputs:
+        s, res = state["dump"]
+        write_outputs(args.dump_outputs, fetch_result(res, w, h))
+        lib.kvz_cuda_ctu_release(enc, s)
     torch.cuda.synchronize()
     seconds = e0.elapsed_time(e1) / 1000.0
     l0, l1 = state["l0"], state["l1"]
@@ -372,7 +425,7 @@ def run_cuda(args, wl):
                 "unit": "GB/s", "frac": ach / peak, "traffic": None, "ms_per_launch": kernel_ms, "algorithmic_bytes_per_launch": alg, "peak_source": peak_src,
                 "note": "the closed-loop CTU search is a chain of dependent decisions (341 CUs per CTU, CTUs in wavefront order): latency bound by "
                         "construction, its HBM traffic is negligible; the HBM-streaming kernel of the north star is roofline_satd_batch "
-                        "(tools/bench_framepass.py, profiles/)"}
+                        "(tools/bench_framepass.py, and roofline_satd_batch in this line)"}
     line = {"metric": METRIC, "value": frames / dev_seconds, "unit": "frames/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
             "ms_per_step": 1000.0 * e2e_seconds / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "u8",
             "data": "synthetic", "config": config_of(wl), "frames_per_step": fps_step,
@@ -441,6 +494,8 @@ def main():
     ap.add_argument("--owf", type=int, default=0, help="pictures the encoder keeps in flight (CUDA arm)")
     ap.add_argument("--slots", type=int, default=0, help="pictures in flight of the device-only leg")
     ap.add_argument("--sample-frames", type=int, default=0)
+    ap.add_argument("--dump-outputs", metavar="DIR", default="",
+                    help="write the device results of ONE picture, the last of the last timed step, to DIR/<name>.npy")
     args = ap.parse_args()
     wl = WORKLOADS[args.workload]
     if args.impl == "reference":

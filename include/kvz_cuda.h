@@ -1,6 +1,6 @@
 /*
- * kvz_cuda.h -- C ABI of libkvzcuda.so: a B200 (sm_100a) "cuda" strategy for Kvazaar's
- * per-CTU strategy kernels (reference: /root/reference/src/strategies, SURVEY.md section 8).
+ * kvz_cuda.h -- C ABI of libkvzcuda.so: an H100 (sm_90a) "cuda" strategy for Kvazaar's
+ * per-CTU strategy kernels (reference: Kvazaar's src/strategies, SURVEY.md section 8).
  *
  * Plain C, no reference headers, no torch types: pointers, sizes and small POD structs only.
  * Three layers, bottom-up:

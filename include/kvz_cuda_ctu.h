@@ -2,7 +2,7 @@
  * kvz_cuda_ctu.h -- C ABI of the device-resident CTU search driver (SURVEY.md §8f rank 2, VERDICT r1 item 1).
  *
  * Replaces, for all-intra pictures, the per-CTU work of the reference's CTU job
- * (encoder_state_worker_encode_lcu, /root/reference/src/encoderstate.c:636-773) up to the point where the bits are
+ * (encoder_state_worker_encode_lcu, src/encoderstate.c:636-773) up to the point where the bits are
  * written:
  *     kvz_search_lcu            src/search.c:1209-1250        (mode decision, reconstruction, coefficients)
  *     kvz_filter_deblock_lcu    src/filter.c:783-792

@@ -1,4 +1,4 @@
-"""kvazaar_b200 -- B200 (sm_100a) "cuda" strategy kernels for Kvazaar's per-CTU hot path.
+"""kvazaar_b200 -- H100 (sm_90a) "cuda" strategy kernels for Kvazaar's per-CTU hot path.
 
 The product is the C-ABI shared library ``libkvzcuda.so`` (include/kvz_cuda.h); this package is the thin
 Python plumbing used by the tests and bench.py: it loads the library with ctypes and passes torch CUDA

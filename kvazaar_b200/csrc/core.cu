@@ -76,8 +76,8 @@ int kvz_cuda_init(int device)
   KVZC_CHECK(cudaSetDevice(device));
   cudaDeviceProp prop;
   KVZC_CHECK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) {
-    set_error("libkvzcuda is built for sm_100a only; device %d is sm_%d%d", device, prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0) {
+    set_error("libkvzcuda is built for sm_90a (H100) only; device %d is sm_%d%d", device, prop.major, prop.minor);
     return KVZ_CUDA_E_NODEVICE;
   }
   g_sm_count = prop.multiProcessorCount;

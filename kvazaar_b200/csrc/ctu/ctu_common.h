@@ -1,7 +1,7 @@
 // ctu_common.h -- types, tables and the execution model of the device-resident CTU search driver (SURVEY §8f rank 2).
 //
 // ONE source, two compilations:
-//   * nvcc, sm_100a: the product.  One CTA (four warps) owns one CTU at a time; every function is called by ALL threads
+//   * nvcc, sm_90a: the product.  One CTA (four warps) owns one CTU at a time; every function is called by ALL threads
 //     of the CTA with uniform control flow unless it takes a Team (ctu_leaf.h): then the CTA's warps run independent
 //     transform-unit jobs side by side and synchronise inside their warp only.  Scalar decisions live in a
 //     shared-memory state block that only the leader (lane 0 of one warp) mutates between barriers -- and every thread

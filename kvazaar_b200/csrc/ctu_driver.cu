@@ -265,8 +265,7 @@ kvz_cuda_ctu_enc *kvz_cuda_ctu_open(const kvz_cuda_ctu_config *cfg, int slots)
   }
   e->diag_launches = getenv("KVZ_CUDA_CTU_DIAG") != nullptr;
   // persistent CTAs per picture: 40 % of the widest diagonal (the average wavefront is about half of it; a smaller grid
-  // leaves fewer CTAs waiting idle and lets more pictures be resident at once -- measured best at 1080p, flat at 2160p,
-  // profiles/r02_grid_sweep.log); KVZ_CUDA_CTU_GRID overrides
+  // leaves fewer CTAs waiting idle and lets more pictures be resident at once); KVZ_CUDA_CTU_GRID overrides
   e->grid = e->diag_launches ? e->max_diag : (e->max_diag * 2 + 4) / 5;
   if (e->grid < 1) e->grid = 1;
   if (const char *g = getenv("KVZ_CUDA_CTU_GRID")) { const int v = atoi(g); if (v > 0 && !e->diag_launches) e->grid = v < e->max_diag ? v : e->max_diag; }

@@ -148,7 +148,7 @@ int kvz_cuda_dequant_batch(const kvz_cuda_quant_params *p, const int16_t *q_coef
   KVZC_ARG(coef && q_coef && (n == 4 || n == 8 || n == 16 || n == 32));
   if (count == 0) return 0;
   const long total = (long)count * n * n;
-  long gl = (total + 255) / 256; if (gl > 148L * 16) gl = 148L * 16;
+  long gl = (total + 255) / 256; if (gl > (long)g_sm_count * 16) gl = (long)g_sm_count * 16;
   const int grid = (int)gl;
   dequant_kernel<<<grid, 256, 0, as_stream(stream)>>>(*p, q_coef, coef, n, type, total);
   KVZC_LAUNCHED();

@@ -856,7 +856,7 @@ static int fp_run_dev_t(kvz_cuda_frame_pass *fp, const void *src_dev, const void
   fp_mark(fp, 39, st);
   // ---- picture checksum of the filtered planes ----
   if constexpr (BD == 8) {
-    checksum3_kernel<<<dim3(148, 3), 256, 0, st>>>(pl, ck_scratch, B + L.checksum);
+    checksum3_kernel<<<dim3(g_sm_count, 3), 256, 0, st>>>(pl, ck_scratch, B + L.checksum);
     KVZC_LAUNCHED();
   } else {
     for (int color = 0; color < 3; ++color)

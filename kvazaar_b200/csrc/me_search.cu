@@ -131,7 +131,7 @@ extern "C" int kvz_cuda_me_search_batch(const kvz_cuda_me_params *p, const void 
   if (int e = check_args(p, cur_dev, cur_stride, ref_dev, ref_stride, pus_dev, count, out_dev)) return e;
   if (count == 0) return 0;
   const int ctas = (count + kWarpsPerCta - 1) / kWarpsPerCta;
-  const int cap = kvzc::g_sm_count > 0 ? kvzc::g_sm_count * 16 : 148 * 16;     // 16 CTAs of 4 warps per SM; more PUs loop
+  const int cap = kvzc::g_sm_count > 0 ? kvzc::g_sm_count * 16 : 132 * 16;     // 16 CTAs of 4 warps per SM; more PUs loop
   const int grid = ctas < cap ? ctas : cap;
   const cudaStream_t st = kvzc::as_stream(stream);
   const dim3 block(kWarpsPerCta * 32);
@@ -219,7 +219,7 @@ extern "C" int kvz_cuda_me_frac_search_batch(const kvz_cuda_me_params *p, int fm
   KVZC_ARG(fme_level >= 1 && fme_level <= 4);
   if (count == 0) return 0;
   const int ctas = (count + kWarpsPerCta - 1) / kWarpsPerCta;
-  const int cap = kvzc::g_sm_count > 0 ? kvzc::g_sm_count * 16 : 148 * 16;
+  const int cap = kvzc::g_sm_count > 0 ? kvzc::g_sm_count * 16 : 132 * 16;
   const int grid = ctas < cap ? ctas : cap;
   if (p->bitdepth == 8)
     me_frac_kernel<uint8_t><<<grid, kWarpsPerCta * 32, 0, kvzc::as_stream(stream)>>>(*p, fme_level, (const uint8_t *)cur_dev, cur_stride,
@@ -268,7 +268,7 @@ extern "C" int kvz_cuda_me_merge_cost_batch(const kvz_cuda_me_params *p, const k
     for (int i = 0; i < 16; ++i) KVZC_ARG(refs->ref_LX[l][i] < 16);
   if (count == 0) return 0;
   const int ctas = (count + kWarpsPerCta - 1) / kWarpsPerCta;
-  const int cap = kvzc::g_sm_count > 0 ? kvzc::g_sm_count * 16 : 148 * 16;
+  const int cap = kvzc::g_sm_count > 0 ? kvzc::g_sm_count * 16 : 132 * 16;
   const int grid = ctas < cap ? ctas : cap;
   if (p->bitdepth == 8)
     me_merge_kernel<uint8_t><<<grid, kWarpsPerCta * 32, 0, kvzc::as_stream(stream)>>>(*p, *refs, (const uint8_t *)cur_dev, cur_stride, pus_dev, count, out_dev);
@@ -288,7 +288,7 @@ extern "C" int kvz_cuda_me_bipred_batch(const kvz_cuda_me_params *p, const kvz_c
     for (int i = 0; i < 16; ++i) KVZC_ARG(refs->ref_LX[l][i] < 16);
   if (count == 0) return 0;
   const int ctas = (count + kWarpsPerCta - 1) / kWarpsPerCta;
-  const int cap = kvzc::g_sm_count > 0 ? kvzc::g_sm_count * 16 : 148 * 16;
+  const int cap = kvzc::g_sm_count > 0 ? kvzc::g_sm_count * 16 : 132 * 16;
   const int grid = ctas < cap ? ctas : cap;
   if (p->bitdepth == 8)
     me_bipred_kernel<uint8_t><<<grid, kWarpsPerCta * 32, 0, kvzc::as_stream(stream)>>>(*p, *refs, (const uint8_t *)cur_dev, cur_stride, pus_dev, count, out_dev);
@@ -309,7 +309,7 @@ extern "C" int kvz_cuda_me_predict_batch(const kvz_cuda_me_params *p, const kvz_
   for (int i = 0; i < 16; ++i) KVZC_ARG((refs->y[i] == nullptr) == (refs->u[i] == nullptr) && (refs->y[i] == nullptr) == (refs->v[i] == nullptr));
   if (count == 0) return 0;
   const int ctas = (count + kWarpsPerCta - 1) / kWarpsPerCta;
-  const int cap = kvzc::g_sm_count > 0 ? kvzc::g_sm_count * 16 : 148 * 16;
+  const int cap = kvzc::g_sm_count > 0 ? kvzc::g_sm_count * 16 : 132 * 16;
   const int grid = ctas < cap ? ctas : cap;
   if (p->bitdepth == 8)
     me_predict_kernel<uint8_t><<<grid, kWarpsPerCta * 32, 0, kvzc::as_stream(stream)>>>(*p, *refs, pus_dev, count, (uint8_t *)pred_y_dev, (uint8_t *)pred_u_dev, (uint8_t *)pred_v_dev);

@@ -311,9 +311,8 @@ int kvz_cuda_satd_nxn_batch(int n, int bitdepth, const void *a, const void *b, i
   KVZC_REQUIRE_DEVICE();
   KVZC_ARG(a && b && out && count >= 0);
   if (bitdepth == 8 && n == 8 && count >= 4096 && (((uintptr_t)a | (uintptr_t)b) & 15) == 0) {
-    // KVZ_CUDA_SATD_TMA=1 selects the persistent TMA-fed variant (satd_tma.cu).  Measured on B200 (profiles/): the
-    // plain 128-bit-load kernel is faster (it keeps 3x more warps in flight for this issue-bound arithmetic), so
-    // it stays the default.
+    // KVZ_CUDA_SATD_TMA=1 selects the persistent TMA-fed variant (satd_tma.cu).  The plain 128-bit-load kernel keeps
+    // 3x more warps in flight for this issue-bound arithmetic, so it stays the default (tools/time_satd.py times both).
     static const bool tma = getenv("KVZ_CUDA_SATD_TMA") != nullptr;
     if (tma) return satd8_tma((const uint8_t *)a, (const uint8_t *)b, count, out, as_stream(stream));
   }

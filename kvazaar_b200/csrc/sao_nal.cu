@@ -257,7 +257,7 @@ int kvz_cuda_array_checksum(int bitdepth, const void *data, int height, int widt
   KVZC_CHECK(cudaMemsetAsync(scratch, 0, 8, st));
   const long total = (long)height * width;
   long g = (total + 256 * 16 - 1) / (256 * 16);
-  const int grid = (int)(g < 1 ? 1 : (g > 148 * 8 ? 148 * 8 : g));
+  const int grid = (int)(g < 1 ? 1 : (g > g_sm_count * 8 ? g_sm_count * 8 : g));
   if (bitdepth == 8) checksum_kernel<uint8_t><<<grid, 256, 0, st>>>((const uint8_t *)data, height, width, stride, scratch, out4);
   else checksum_kernel<uint16_t><<<grid, 256, 0, st>>>((const uint16_t *)data, height, width, stride, scratch, out4);
   KVZC_LAUNCHED();

@@ -1,6 +1,6 @@
 """The bodies of the motion-search `-m gpu` tests, run on the CPU against the host build of the device code through a
 stand-in module (tests/_fake_kb.py): a typo, a wrong view or a swapped argument in a GPU-only test would otherwise surface
-only on the B200 box.  Validates the test code and tools/bench_me.py's bookkeeping, not the device."""
+only on the GPU machine.  Validates the test code and tools/bench_me.py's bookkeeping, not the device."""
 import pytest
 import torch
 
@@ -41,8 +41,9 @@ def test_fractional_test_bodies(kb, ref, ref10):
         B.test_cuda_motion_compensation_matches_golden_and_reference(kb, name, ref, ref10)
 
 
-def test_bench_me_bookkeeping(kb, monkeypatch):
-    """tools/bench_me.py's measure() with the stand-in: every stage reports `identical`"""
+def test_bench_me_bookkeeping(kb, ref, monkeypatch):
+    """tools/bench_me.py's measure() with the stand-in: every stage reports `identical` (measure() checks against the
+    compiled reference, like the test bodies above)"""
     import time
     import kvazaar_b200
     import bench_me

@@ -130,7 +130,7 @@ LATER = sorted(set(CASES) - set(GPU_FIRST_RUN_DONE))
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", [n for n in LATER if "satd_final" not in n])
 def test_cuda_integer_search_cases_added_later(cuda_lib, name, ref, ref10):
-    """tz and full search cases of tools/me_cases.py (added after the integer kernel's first B200 run; same check_mv primitive)"""
+    """tz and full search cases of tools/me_cases.py (added after the first search cases; same check_mv primitive)"""
     check_cuda_case(cuda_lib, name, ref, ref10)
 
 
@@ -276,8 +276,6 @@ def test_tenbit_host_program_matches_reference_cli(tmp_path):
 
 
 @pytest.mark.gpu
-@pytest.mark.xfail(strict=False, reason="first hardware run of the 10-bit per-call strategy path inside an encode: the 10-bit kernels are covered "
-                                        "function by function (tests/test_10bit.py), the 10-bit glue build has never met a GPU")
 def test_tenbit_bitstream_identical_with_cuda_strategies(cuda_lib, tmp_path):
     """VERDICT r1 item 3: the 10-bit reference encoder (inter, FME, bipred) with every strategy pointer bound to CUDA"""
     import re

@@ -57,7 +57,7 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "fallback (H100 SXM data sheet, HBM3)"
 
 
 def synth_frames(n):
@@ -302,12 +302,6 @@ def run_cuda(args):
     # per-LAUNCH time of each kernel (chroma stages hold two launches: U and V; deblocking two passes)
     per_launch = [stage_ms[i] / (2 if names[i].startswith("recon_chroma") or names[i] == "deblock" else 1) for i in range(NST)]
     dom = int(np.argmax(per_launch))
-    ncu = {}
-    for fn in ("r01_ncu_summary.json", "r01b_ncu_summary.json"):      # later captures override earlier ones
-        try:
-            ncu.update(json.load(open(os.path.join(ROOT, "profiles", fn))))
-        except Exception:
-            pass
 
     def alg_bytes(name):
         """Bytes one launch must move through HBM (DESIGN.md section 4)."""
@@ -343,18 +337,15 @@ def run_cuda(args):
                  "rdoq_chroma": "rdoq_grid_kernel", "bits_luma": "coeff_cost_grid_kernel", "bits_chroma": "coeff_cost_grid_kernel",
                  "sao_stats_decide": "sao_ctu_kernel", "deblock": "deblock_pass_kernel"}.get(names[dom].rsplit("_w", 1)[0], names[dom])
         roof = {"kernel": f"{kname} [{names[dom]}]", "bound": "hbm", "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak,
-                "traffic": ncu.get(names[dom], {}).get("dram_bytes_per_launch"), "ms_per_launch": per_launch[dom],
+                "traffic": None, "ms_per_launch": per_launch[dom],
                 "algorithmic_bytes_per_launch": alg, "peak_source": peak_src,
-                "note": ("RDOQ is HM's serial per-TU chain (one lane of a warp walks the scan in double precision): latency bound, "
-                         f"ncu {ncu.get(names[dom], {}).get('issue_active_pct', 'n/a')}% issue-active at "
-                         f"{ncu.get(names[dom], {}).get('warps_active_pct', 'n/a')}% warps-active; "
+                "note": ("RDOQ is HM's serial per-TU chain (one lane of a warp walks the scan in double precision): latency bound; "
                          if names[dom].startswith("rdoq") else
-                         "fused per-block kernels keep predictions / transforms on chip: they are instruction-issue bound "
-                         f"(ncu: {ncu.get(names[dom], {}).get('issue_active_pct', 'n/a')}% issue-active), not HBM bound; ")
+                         "fused per-block kernels keep predictions / transforms on chip: they are instruction-issue bound, not HBM bound; ")
                         + "roofline_satd_batch is the HBM-streaming kernel of the north star"}
 
     # ---- the batched SATD kernel of the north_star (block pairs streamed from HBM), inputs > L2
-    n_pairs = 4 * 1024 * 1024            # 4M 8x8 pairs = 512 MiB of pixels > 126 MB L2
+    n_pairs = 4 * 1024 * 1024            # 4M 8x8 pairs = 512 MiB of pixels > 50 MB L2
     g = torch.Generator(device="cuda").manual_seed(7)
     a = torch.randint(0, 256, (n_pairs * 64,), dtype=torch.uint8, device="cuda", generator=g)
     b = torch.randint(0, 256, (n_pairs * 64,), dtype=torch.uint8, device="cuda", generator=g)
@@ -377,7 +368,6 @@ def run_cuda(args):
                  "unit": "GB/s", "frac": ach_satd / peak, "traffic": None, "ms_per_launch": ms_satd, "pairs_per_launch": n_pairs,
                  "algorithmic_bytes_per_launch": alg_satd, "peak_source": peak_src, "checksum": int(out.to(torch.int64).sum()),
                  "ms_per_launch_min_median_max": [round(float(np.min(per)), 5), round(float(np.median(per)), 5), round(float(np.max(per)), 5)]}
-    roof_satd["traffic"] = ncu.get("satd_nxn_kernel_8", {}).get("dram_bytes_per_launch")
     del a, b
 
     if rank == 0:
@@ -386,7 +376,7 @@ def run_cuda(args):
                 "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "u8" if BITDEPTH == 8 else "u16", "data": "synthetic",
                 "config": {"workload": WORKLOAD, "frames_per_step": fps_step, "frames_in_flight": inflight, "parallelism": f"frames/{world}",
                            "l2": f"working set per step ({fps_step} distinct {passes[0].frame_bytes / 1e6:.1f} MB frames + {inflight} result/scratch blobs of "
-                                 f"{passes[0].host_bytes / 1e6:.0f}+ MB each) exceeds the 126 MB L2"},
+                                 f"{passes[0].host_bytes / 1e6:.0f}+ MB each) exceeds the 50 MB L2"},
                 "e2e": {"value": e2e, "unit": "frames/s", "h2d_bytes_per_step": fps_step * passes[0].frame_bytes,
                         "d2h_bytes_per_step": fps_step * d2h_compact, "ms_per_step": ms_e2e / args.steps,
                         "result": "compact: blob head + bitmap + non-zero 32-byte coefficient chunks (lossless)" if compact_ok

@@ -48,7 +48,7 @@ def measure(res="1920x1080", pu=16, algo="hexbs", bitdepth=8, iters=20, fme_leve
     p.ime_algorithm = {"hexbs": 0, "tz": 1, "full8": 3, "full16": 4, "dia": 7}[algo]
     d_cur, d_ref, d_pus = kb.to_dev(cur), kb.to_dev(rf), kb.to_dev(pus)
     px = 1 if bitdepth == 8 else 2
-    peak = 6650.0
+    peak = 3350.0     # H100 SXM data sheet (HBM3) unless measured
     mp = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(mp):
         peak = float(json.load(open(mp))["hbm_gbs"])

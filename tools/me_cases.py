@@ -353,8 +353,8 @@ def run_frac_reference(ref_shim, p, level, cur, ref, pus):
 CASES["hexbs_satd_final"] = dict(w=208, h=136, bd=8, algo=0, steps=-1, et=2, mvc=0, wpp=1, delay=8, qp=32, seed=17, n=300, satd_final=1)
 CASES["dia_satd_final_10bit"] = dict(w=136, h=72, bd=10, algo=7, steps=-1, et=1, mvc=0, wpp=0, delay=0, qp=27, seed=18, n=200, satd_final=1)
 
-# the search cases whose -m gpu test has already passed on a B200 (profiles/r02_test_me_gpu.log); the GPU tests of the cases
-# added after that run live in tests/test_zz_me_frac.py, which sorts last
+# the search cases of tests/test_me_search.py's -m gpu tests; the GPU tests of the cases added later live in
+# tests/test_zz_me_frac.py, which sorts last
 GPU_FIRST_RUN_DONE = ["dia_10bit_margin", "dia_et_off_steps3", "dia_et_sensitive", "hexbs_10bit", "hexbs_et_off_margin", "hexbs_et_on_wpp_sao",
                       "hexbs_et_sensitive", "hexbs_noisy", "hexbs_steps0", "hexbs_steps2_frame"]
 
