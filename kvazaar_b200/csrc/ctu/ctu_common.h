@@ -64,7 +64,7 @@ extern __shared__ __align__(16) unsigned char ctu_smem_raw[];
 
 // Phase profile (diagnostic build, make PROF=1): cycles of the leader thread per phase, summed over all CTUs.
 enum { PR_LOAD, PR_SEARCH, PR_STORE, PR_DEBLOCK, PR_SAO, PR_TRACK, PR_REFS, PR_SATD, PR_REPLAY, PR_PREDICT, PR_QRES, PR_FWD, PR_RDOQ, PR_QUANT,
-       PR_INV, PR_SSD, PR_COST, PR_COPY, PR_COEFFCOST, PR_WAIT, PR_CHROMA, PR_RDO_LOOP, PR_N };
+       PR_INV, PR_SSD, PR_COST, PR_COPY, PR_COEFFCOST, PR_WAIT, PR_CHROMA, PR_RDO_LOOP, PR_WRITEBACK, PR_N };
 #if defined(KVZ_CTU_PROF) && defined(__CUDA_ARCH__)
 #define PROF_T0(id) const long long prof_t0_##id = clock64()
 #define PROF_ADD(S, id) do { if (CTU_TID == CTU_LEADER_TID) (S)->prof[id] += clock64() - prof_t0_##id; } while (0)

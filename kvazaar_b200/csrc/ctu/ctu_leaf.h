@@ -23,8 +23,17 @@ namespace kvzctu {
 #endif
 
 // ------------------------------------------------------------------------------------------------ work memory
+// Reconstruction and levels of the RDO candidates of the CU searched last (search_cu_intra), so that the winner's are
+// written back instead of computed a second time.  Luma: unit (candidate * alternatives + alternative), the alternatives
+// being transform / transform skip of a 4x4 unit; chroma: unit (candidate).  Units of the CU's size, back to back.
+#define CTU_RDO_CANDS 6             // search_intra_rdo: at most 3 rough-search modes (2 above depth 4) and the 3 MPMs
+struct CandStore {
+  uint8_t rec_y[CTU_RDO_CANDS * 1024], rec_c[2][CTU_RDO_CANDS * 256];
+  int16_t q_y[CTU_RDO_CANDS * 1024], q_c[2][CTU_RDO_CANDS * 256];
+};
 struct CtuWork {                    // per resident CTU, global memory (L2 resident)
   LcuStore store[5];
+  CandStore cand;
   uint8_t src_y[64 * 64], src_u[32 * 32], src_v[32 * 32];       // lcu->ref
   // border references from the neighbouring CTUs, index 0 = top-left corner sample (lcu->top_ref / left_ref)
   uint8_t top_y[100], top_u[52], top_v[52], left_y[100], left_u[52], left_v[52];

@@ -18,8 +18,9 @@
 // out: the rough search evaluates the SATD of all 35 modes in one data-parallel phase and then replays the reference's
 // halving search on the table; the RDO candidates of search_intra_rdo and the colours of a CU are independent
 // transform-unit jobs that run one per warp (for_tu_tasks) with private reconstructions, and only SSD / cbf / exact
-// coefficient bits come back to the leader, which assembles the costs in the reference's order; the cost walks that adapt
-// the context models stay serial on the leader.
+// coefficient bits come back to the leader, which assembles the costs in the reference's order; each job keeps its
+// reconstruction and levels in CtuWork, and the winner's are written back where the reference reconstructs the chosen
+// mode once more; the cost walks that adapt the context models stay serial on the leader.
 #pragma once
 #include "ctu_leaf.h"
 
@@ -37,7 +38,7 @@ struct SearchFrame {
   CabacState pre, post;
 };
 
-struct TuRes { int32_t ssd, has, tr_skip, pad; double bits; };
+struct TuRes { int32_t ssd, has, tr_skip, pad; double bits; uint64_t cg_mask; };
 
 struct CtuS {                       // per-CTA scalar state + scratch; shared memory on the device
   int32_t leader_tid;               // MUST be first: CTU_LEADER_TID reads it through the raw shared-memory symbol
@@ -53,6 +54,7 @@ struct CtuS {                       // per-CTA scalar state + scratch; shared me
   int8_t modes[40];
   double costs[40];
   int32_t n_modes;
+  int8_t cand_modes[CTU_RDO_CANDS]; // the RDO candidates in evaluation order: index into res[] and CtuWork::cand
   int8_t mpm[4];
   int8_t cmodes[8];                 // chroma candidates
   double ccosts[8];
@@ -63,8 +65,8 @@ struct CtuS {                       // per-CTA scalar state + scratch; shared me
   double best_cost;
   SmTables tb;
   LcuLevel lv[5];                   // work tree: CU records here, planes in CtuWork::store
-  TuRes res[8][3];                  // [RDO candidate][colour]
-  TuRes res_ts[8][2];               // [RDO candidate][transform, transform skip] of a 4x4 luma unit
+  TuRes res[CTU_RDO_CANDS][3];      // [RDO candidate][colour]
+  TuRes res_ts[CTU_RDO_CANDS][2];   // [RDO candidate][transform, transform skip] of a 4x4 luma unit
   // the coefficients of the transform units reconstructed last (the CU whose cost is computed next), per colour
   int16_t stage_y[1024], stage_c[2][256];
   int32_t stage_key[3];             // (xl << 16) | (yl << 8) | depth of the staged unit, -1: none
@@ -340,6 +342,56 @@ CTU_FN_NOINLINE void intra_recon_cu(const Ctx &c, LcuLevel *L, int x, int y, int
   } else {
     intra_recon_leaf(c, L, x, y, depth, mode_luma, mode_chroma, cur_cu, 0, refs_valid);
   }
+}
+
+// What intra_recon_cu(mode, with_chroma ? mode : -1, NULL, refs_valid) leaves for the leaf CU at (x, y, depth) that
+// search_cu_intra has just evaluated at rdo >= 2 with `mode` among its RDO candidates, taken from that candidate's
+// results instead of computed again: the candidate's transform-unit jobs had the same references, source, scan and
+// models.  Except chroma at depth 4, which is reconstructed again: the candidate quantised it with the cbf context of
+// tr_depth 1 (pred_cu of search_intra_rdo), the CU's reconstruction uses its record's tr_depth 4 - depth 3 + NxN = 2
+// (rdo.c:919).
+CTU_FN_NOINLINE void write_back_candidate(const Ctx &c, LcuLevel *L, int x, int y, int depth, int mode, bool with_chroma)
+{
+  CtuS *S = c.S;
+  const int xl = x & 63, yl = y & 63;
+  const int last = with_chroma && depth < 4 ? 2 : 0;
+  PROF_T0(PR_WRITEBACK);
+  int cand = 0;
+  while (S->cand_modes[cand] != mode) ++cand;
+  const bool ts_split = depth == 4 && c.cfg->trskip_enable;
+  for (int col = 0; col <= last; ++col) {
+    const int log2n = tu_log2(depth, col), n = 1 << log2n;
+    const int unit = col == 0 ? (ts_split ? 2 * cand + S->res[cand][0].tr_skip : cand) : cand;
+    const uint8_t *kr = (col == 0 ? c.W->cand.rec_y : c.W->cand.rec_c[col - 1]) + unit * n * n;
+    const int16_t *kq = (col == 0 ? c.W->cand.q_y : c.W->cand.q_c[col - 1]) + unit * n * n;
+    const Plane P = plane_of(c.W, L, col);
+    const int sh = col ? 1 : 0;
+    uint8_t *rec = P.rec + (xl >> sh) + (yl >> sh) * P.lw;
+    int16_t *co = P.coeff + zorder(P.lw, xl >> sh, yl >> sh);
+    int16_t *stage = col == 0 ? S->stage_y : S->stage_c[col - 1];
+    #pragma unroll 1
+    for (int e = CTU_TID; e < n * n; e += CTU_NT) {
+      rec[(e >> log2n) * P.lw + (e & (n - 1))] = kr[e];
+      co[e] = kq[e];
+      stage[e] = kq[e];
+    }
+  }
+  CTU_LEADER {
+    CuRec *cu = cu_at(L, xl, yl);
+    for (int col = 0; col <= last; ++col) {
+      const TuRes &r = S->res[cand][col];
+      cbf_clear(&cu->cbf, depth, col);      // (the record holds the cbf bits of the candidate evaluated last)
+      if (r.has) cbf_set(&cu->cbf, depth, col);
+      if (col == 0 && ts_split) cu->tr_skip = (uint8_t)r.tr_skip;
+      S->stage_key[col] = stage_key_of(xl, yl, depth);
+      S->stage_mask[col] = r.cg_mask;
+      S->ssd[0][col] = r.ssd;
+      for (int k = 1; k < 4; ++k) S->ssd[k][col] = 0;
+    }
+  }
+  CTU_SYNC();
+  PROF_ADD(S, PR_WRITEBACK);
+  if (with_chroma && depth == 4) intra_recon_cu(c, L, x, y, depth, -1, mode, NULL, 7);
 }
 
 // ------------------------------------------------------------------------------------------------ RD costs
@@ -620,6 +672,15 @@ CTU_FN_NOINLINE int rough_search_replay(const Ctx &c, int log2w, const int8_t *m
   return n;
 }
 
+// copy of a transform-unit job's reconstruction and levels (team)
+CTU_FN_NOINLINE void keep_unit(const Team &tm, const TuS &tu, uint8_t *kr, int16_t *kq)
+{
+  const uint8_t *r = tu.rec();
+  const int16_t *q = tu.q();
+  #pragma unroll 1
+  for (int e = tm.tid; e < tu.nn; e += tm.nt) { kr[e] = r[e]; kq[e] = q[e]; }
+}
+
 // kvz_search_cu_intra (ref: search_intra.c:806-900): best luma mode of the CU at (x, y, depth) on level L.
 // Result in S->best_mode / S->best_cost.
 CTU_FN_NOINLINE void search_cu_intra(const Ctx &c, LcuLevel *L, int x, int y, int depth)
@@ -694,13 +755,20 @@ CTU_FN_NOINLINE void search_cu_intra(const Ctx &c, LcuLevel *L, int x, int y, in
       int ts = 0;
       if (col == 0 && ts_split) tu_core(tm, &c.S->tb, &S->tb, cfg, S->cabac0.ctx, tu, j, k == 1);
       else ts = tu_eval(tm, &c.S->tb, &S->tb, cfg, S->cabac0.ctx, &S->sc, tu, j);
+      // keep the unit for write_back_candidate (not the chroma of depth 4, which is quantised again: see there)
+      if (col == 0 || depth < 4) {
+        const int unit = col == 0 ? cand * nluma + k : cand;
+        uint8_t *kr = (col == 0 ? c.W->cand.rec_y : c.W->cand.rec_c[col - 1]) + unit * n * n;
+        int16_t *kq = (col == 0 ? c.W->cand.q_y : c.W->cand.q_c[col - 1]) + unit * n * n;
+        keep_unit(tm, tu, kr, kq);
+      }
       if (tm.tid == 0) {
         const TuFixed *fx = tu.fx();
         TuRes *r = (col == 0 && ts_split) ? &S->res_ts[cand][k] : &S->res[cand][col];
         r->ssd = fx->ssd; r->has = fx->has; r->tr_skip = ts;
+        r->cg_mask = (uint64_t)fx->cg_mask[0] | ((uint64_t)fx->cg_mask[1] << 32);
         // coefficient bits of kvz_cu_rd_cost_luma / _chroma: the search models are not adapted here (update == 0)
-        r->bits = fx->has ? coeff_cost_serial(&c.S->tb, &S->tb, cfg, &S->sc, tu.q(), log2n, col ? 2 : 0, j.scan_idx, 0,
-                                              (uint64_t)fx->cg_mask[0] | ((uint64_t)fx->cg_mask[1] << 32)) : 0.0;
+        r->bits = fx->has ? coeff_cost_serial(&c.S->tb, &S->tb, cfg, &S->sc, tu.q(), log2n, col ? 2 : 0, j.scan_idx, 0, r->cg_mask) : 0.0;
       }
       tsync(tm);
     });
@@ -738,7 +806,11 @@ CTU_FN_NOINLINE void search_cu_intra(const Ctx &c, LcuLevel *L, int x, int y, in
     CTU_SYNC();
     PROF_ADD(S, PR_COST);
     checked = S->n_modes;
-    CTU_LEADER { S->n_modes = checked; sort_modes(S->modes, S->costs, checked); }
+    CTU_LEADER {
+      for (int r = 0; r < checked; ++r) S->cand_modes[r] = S->modes[r];
+      S->n_modes = checked;
+      sort_modes(S->modes, S->costs, checked);
+    }
     CTU_SYNC();
   }
   PROF_ADD(S, PR_RDO_LOOP);
@@ -897,6 +969,9 @@ CTU_FN_NOINLINE void search_ctu(const Ctx &c, int cx, int cy)
             CTU_SYNC();
             fill_cu_info(L, xl, yl, cu_width, cur_cu);
             intra_recon_cu(c, L, x, y, d, -1, cur_cu->mode_chroma, NULL, 0);
+          } else if (cfg->rdo >= 2) {
+            // the winner's reconstruction is the one its RDO candidate computed (a leaf: depth >= 1, tr_depth == depth)
+            write_back_candidate(c, L, x, y, d, cur_cu->mode, aligned);
           } else {
             // luma and chroma of the CU are independent: one pass (kvz_intra_recon_cu twice in the reference)
             intra_recon_cu(c, L, x, y, d, cur_cu->mode, aligned ? cur_cu->mode_chroma : -1, NULL, refs_valid);
