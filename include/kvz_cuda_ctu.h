@@ -16,6 +16,13 @@
  *
  * Plain pointers and sizes only; no CUDA or torch types.  Result buffers are pinned host memory owned by the
  * library, valid from kvz_cuda_ctu_wait until kvz_cuda_ctu_release.
+ *
+ * Bit depth: kvz_cuda_ctu_config.bitdepth selects the sample type of every picture buffer crossing this interface --
+ * 0 or 8: uint8_t samples, 10: uint16_t samples (kvz_pixel of a KVZ_BIT_DEPTH=10 build of the reference, values
+ * 0..1023).  Strides and plane widths count samples, not bytes.  The result pointers are `const void *` to samples
+ * of that type.  The source pointers of kvz_cuda_ctu_submit / _submit_device keep their `const uint8_t *` type, so
+ * that providers and callers written for 8 bits build unchanged: at 10 bits the caller passes its uint16_t planes
+ * cast to `const uint8_t *`, and the provider reads uint16_t samples from them.
  */
 #ifndef KVZ_CUDA_CTU_H_
 #define KVZ_CUDA_CTU_H_
@@ -38,7 +45,7 @@ typedef struct kvz_cuda_ctu_config {
   int32_t cu_split_termination;     /* 0 zero, 1 off */
   int32_t intra_rdo_et, combine_intra_cus, intra_chroma_search, full_intra_search;
   int32_t wpp;
-  int32_t pad;
+  int32_t bitdepth;                 /* 0 or 8: 8-bit (uint8_t samples), 10: 10-bit (uint16_t samples); others are rejected */
   double  lambda, lambda_sqrt;      /* state->lambda, state->lambda_sqrt */
 } kvz_cuda_ctu_config;
 
@@ -65,14 +72,14 @@ typedef struct kvz_cuda_ctu_result {
   int32_t pad;
   const int16_t *coeff;             /* per CTU (raster): y[64*64] u[32*32] v[32*32], TUs in z-order (lcu_coeff_t, src/cu.h:292-296) */
   const kvz_cuda_ctu_sao *sao;      /* per CTU: [0] luma, [1] chroma */
-  const uint8_t *rec_y, *rec_u, *rec_v;   /* final picture, stride = width (/2) */
+  const void *rec_y, *rec_u, *rec_v;      /* final picture, stride = width (/2) samples of the configured type */
   const uint8_t *dbg_ctx;           /* per CTU: the 184 context-model bytes the CTU's search started from (may be NULL) */
-  const uint8_t *dbg_y, *dbg_u, *dbg_v;   /* the search's reconstruction before deblocking (may be NULL; verification) */
+  const void *dbg_y, *dbg_u, *dbg_v;      /* the search's reconstruction before deblocking (may be NULL; verification) */
 } kvz_cuda_ctu_result;
 
 typedef struct kvz_cuda_ctu_enc kvz_cuda_ctu_enc;
 
-/* 0 if the configuration is inside the driver's scope (8-bit 4:2:0 all-intra, see csrc/ctu/ctu_search.h) */
+/* 0 if the configuration is inside the driver's scope (8- or 10-bit 4:2:0 all-intra, see csrc/ctu/ctu_search.h) */
 int kvz_cuda_ctu_config_supported(const kvz_cuda_ctu_config *cfg);
 /* slots = pictures that may be in flight at once (submitted, not yet released).  NULL on failure (kvz_cuda_last_error). */
 kvz_cuda_ctu_enc *kvz_cuda_ctu_open(const kvz_cuda_ctu_config *cfg, int slots);
@@ -90,7 +97,7 @@ typedef struct kvz_cuda_ctu_device_result {
   const kvz_cuda_ctu_cu *cu;
   const int16_t *coeff;
   const kvz_cuda_ctu_sao *sao;
-  const uint8_t *rec;               /* final picture: Y, U, V planes back to back, stride = width (/2) */
+  const void *rec;                  /* final picture: Y, U, V planes back to back, stride = width (/2) samples */
   int32_t cu_stride, width_in_lcu, height_in_lcu;
   float search_kernel_ms;           /* device time of the picture's search launch(es), CUDA events on its stream */
 } kvz_cuda_ctu_device_result;

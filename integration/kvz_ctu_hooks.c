@@ -17,6 +17,8 @@
  *   KVZ_CTU_SLOTS    = picture slots of the provider (default and minimum: owf + 1, the pictures the encoder keeps in
  *                      flight -- a worker blocked on a busy slot could otherwise starve the pictures that hold the slots)
  * Without KVZ_CTU_PROVIDER, or when the configuration is outside the driver's scope, every hook falls through.
+ * The same source serves the 8-bit and the 10-bit build of the reference (KVZ_BIT_DEPTH): pictures cross the driver's
+ * interface as kvz_pixel samples, and kvz_cuda_ctu_config.bitdepth tells the provider which.
  */
 #define _GNU_SOURCE
 #include <dlfcn.h>
@@ -84,6 +86,7 @@ static void fill_config(const encoder_state_t *state, kvz_cuda_ctu_config *c)
   c->intra_rdo_et = cfg->intra_rdo_et; c->combine_intra_cus = cfg->combine_intra_cus;
   c->intra_chroma_search = cfg->intra_chroma_search; c->full_intra_search = cfg->full_intra_search;
   c->wpp = cfg->wpp;
+  c->bitdepth = ctrl->bitdepth;
   c->lambda = state->lambda; c->lambda_sqrt = state->lambda_sqrt;
 }
 
@@ -94,7 +97,7 @@ static int config_in_scope(const encoder_state_t *state)
 {
   const encoder_control_t *ctrl = state->encoder_control;
   const kvz_config *cfg = &ctrl->cfg;
-  if (KVZ_BIT_DEPTH != 8 || ctrl->bitdepth != 8 || ctrl->chroma_format != KVZ_CSP_420) return 0;
+  if (ctrl->bitdepth != KVZ_BIT_DEPTH || (ctrl->bitdepth != 8 && ctrl->bitdepth != 10) || ctrl->chroma_format != KVZ_CSP_420) return 0;
   if (cfg->intra_period != 1) return 0;
   if (cfg->lossless || cfg->tr_depth_intra != 0 || cfg->rdo > 3) return 0;
   if (ctrl->scaling_list.enable) return 0;
@@ -171,14 +174,16 @@ static job_t *job_get(encoder_state_t *state, int x, int y)
     static _Thread_local uint8_t ctx[184];
     _Static_assert(sizeof(state->cabac.ctx) == 184, "cabac context image");
     memcpy(ctx, &state->cabac.ctx, 184);
-    j->slot = g_prov.submit(g_enc, src->y, src->u, src->v, src->stride, src->stride / 2, ctx, state->lambda, state->lambda_sqrt, state->qp);
+    j->slot = g_prov.submit(g_enc, (const uint8_t *)src->y, (const uint8_t *)src->u, (const uint8_t *)src->v, src->stride, src->stride / 2, ctx, state->lambda, state->lambda_sqrt, state->qp);
     if (j->slot < 0 || g_prov.wait(g_enc, j->slot, &j->res) != 0) { fprintf(stderr, "kvz-ctu: device search failed\n"); abort(); }
     if (!g_verify) {
       kvz_picture *rec = frame->rec;
-      for (int r = 0; r < frame->height; ++r) memcpy(rec->y + (size_t)r * rec->stride, j->res.rec_y + (size_t)r * frame->width, frame->width);
+      const kvz_pixel *ry = j->res.rec_y, *ru = j->res.rec_u, *rv = j->res.rec_v;
+      const size_t w = frame->width, wc = w / 2;
+      for (int r = 0; r < frame->height; ++r) memcpy(rec->y + (size_t)r * rec->stride, ry + r * w, w * sizeof(kvz_pixel));
       for (int r = 0; r < frame->height / 2; ++r) {
-        memcpy(rec->u + (size_t)r * (rec->stride / 2), j->res.rec_u + (size_t)r * (frame->width / 2), frame->width / 2);
-        memcpy(rec->v + (size_t)r * (rec->stride / 2), j->res.rec_v + (size_t)r * (frame->width / 2), frame->width / 2);
+        memcpy(rec->u + (size_t)r * (rec->stride / 2), ru + r * wc, wc * sizeof(kvz_pixel));
+        memcpy(rec->v + (size_t)r * (rec->stride / 2), rv + r * wc, wc * sizeof(kvz_pixel));
       }
     }
   }
@@ -235,17 +240,18 @@ void __wrap_kvz_search_lcu(encoder_state_t *state, int x, int y, const yuv_t *ho
       }
     if (j->res.dbg_y) {
       const kvz_picture *rec = frame->rec;
+      const kvz_pixel *dy = j->res.dbg_y, *du = j->res.dbg_u, *dv = j->res.dbg_v;
       int done = 0;
       for (int yy = 0; yy < y_max && !done; ++yy)
         for (int xx = 0; xx < x_max; ++xx)
-          if (rec->y[(size_t)(y + yy) * rec->stride + x + xx] != j->res.dbg_y[(size_t)(y + yy) * frame->width + x + xx]) {
-            report("rec_y (before deblocking)", x, y, xx, yy, rec->y[(size_t)(y + yy) * rec->stride + x + xx], j->res.dbg_y[(size_t)(y + yy) * frame->width + x + xx]); done = 1; break; }
+          if (rec->y[(size_t)(y + yy) * rec->stride + x + xx] != dy[(size_t)(y + yy) * frame->width + x + xx]) {
+            report("rec_y (before deblocking)", x, y, xx, yy, rec->y[(size_t)(y + yy) * rec->stride + x + xx], dy[(size_t)(y + yy) * frame->width + x + xx]); done = 1; break; }
       done = 0;
       for (int yy = 0; yy < y_max / 2 && !done; ++yy)
         for (int xx = 0; xx < x_max / 2; ++xx) {
           const size_t a = (size_t)(y / 2 + yy) * (rec->stride / 2) + x / 2 + xx, b = (size_t)(y / 2 + yy) * (frame->width / 2) + x / 2 + xx;
-          if (rec->u[a] != j->res.dbg_u[b]) { report("rec_u (before deblocking)", x, y, xx, yy, rec->u[a], j->res.dbg_u[b]); done = 1; break; }
-          if (rec->v[a] != j->res.dbg_v[b]) { report("rec_v (before deblocking)", x, y, xx, yy, rec->v[a], j->res.dbg_v[b]); done = 1; break; }
+          if (rec->u[a] != du[b]) { report("rec_u (before deblocking)", x, y, xx, yy, rec->u[a], du[b]); done = 1; break; }
+          if (rec->v[a] != dv[b]) { report("rec_v (before deblocking)", x, y, xx, yy, rec->v[a], dv[b]); done = 1; break; }
         }
     }
     for (int i = 0; i < 4096; ++i) if (state->coeff->y[i] != co[i]) { report("coeff_y", x, y, i, 0, state->coeff->y[i], co[i]); break; }

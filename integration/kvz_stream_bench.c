@@ -8,6 +8,8 @@
  *                                                          (integration/kvz_ctu_hooks.c); KVZ_CTU_PROVIDER selects
  *                                                          libkvzcuda.so
  * so both arms of bench.py measure the same loop, the one src/encmain.c:551-745 runs minus the file reader thread.
+ * Built against the 10-bit reference (KVZ_BIT_DEPTH=10: kvz_stream_bench_{ref,ctu}_10b) the clip holds 16-bit
+ * little-endian samples, kvz_pixel as the reference's own reader takes them.
  *
  *   kvz_stream_bench clip.yuv WxH out.hevc frames_per_step steps warmup cooldown [key=value ...]   (keys as in kvazaar --help)
  *
@@ -42,7 +44,7 @@ int main(int argc, char **argv)
   int w = 0, h = 0;
   if (sscanf(res, "%dx%d", &w, &h) != 2 || fps_step < 1 || steps < 1 || warmup < 0 || cooldown < 0) { fprintf(stderr, "bad arguments\n"); return 2; }
 
-  const kvz_api *api = kvz_api_get(8);
+  const kvz_api *api = kvz_api_get(KVZ_BIT_DEPTH);
   kvz_config *cfg = api->config_alloc();
   api->config_init(cfg);
   char num[32];
@@ -59,7 +61,7 @@ int main(int argc, char **argv)
   /* the clip, resident in host memory */
   FILE *fi = fopen(in, "rb");
   if (!fi) { fprintf(stderr, "cannot open %s\n", in); return 1; }
-  const size_t ysz = (size_t)w * h, csz = ysz / 4, fsz = ysz + 2 * csz;
+  const size_t ysz = (size_t)w * h, csz = ysz / 4, fsz = (ysz + 2 * csz) * sizeof(kvz_pixel);    /* samples, samples, bytes */
   fseek(fi, 0, SEEK_END);
   const long clip_frames = ftell(fi) / (long)fsz;
   fseek(fi, 0, SEEK_SET);
@@ -81,11 +83,11 @@ int main(int argc, char **argv)
     kvz_picture *pic = NULL;
     if (fed < total) {
       pic = api->picture_alloc(w, h);
-      const unsigned char *f = clip + (size_t)(fed % clip_frames) * fsz;
-      for (int r = 0; r < h; ++r) memcpy(pic->y + (size_t)r * pic->stride, f + (size_t)r * w, (size_t)w);
+      const kvz_pixel *f = (const kvz_pixel *)(clip + (size_t)(fed % clip_frames) * fsz);
+      for (int r = 0; r < h; ++r) memcpy(pic->y + (size_t)r * pic->stride, f + (size_t)r * w, (size_t)w * sizeof(kvz_pixel));
       for (int r = 0; r < h / 2; ++r) {
-        memcpy(pic->u + (size_t)r * (pic->stride / 2), f + ysz + (size_t)r * (w / 2), (size_t)w / 2);
-        memcpy(pic->v + (size_t)r * (pic->stride / 2), f + ysz + csz + (size_t)r * (w / 2), (size_t)w / 2);
+        memcpy(pic->u + (size_t)r * (pic->stride / 2), f + ysz + (size_t)r * (w / 2), (size_t)w / 2 * sizeof(kvz_pixel));
+        memcpy(pic->v + (size_t)r * (pic->stride / 2), f + ysz + csz + (size_t)r * (w / 2), (size_t)w / 2 * sizeof(kvz_pixel));
       }
       if (fed == 0 && first_timed == 0) t_start = t_prev = now();
       ++fed;

@@ -75,6 +75,18 @@ enum { PR_LOAD, PR_SEARCH, PR_STORE, PR_DEBLOCK, PR_SAO, PR_TRACK, PR_REFS, PR_S
 
 namespace kvzctu {
 
+// ---------------------------------------------------------------------------------------------- sample type
+// The algorithm is compiled once per sample type: uint8_t for 8-bit, uint16_t for 10-bit pictures (kvz_pixel of the
+// reference's KVZ_BIT_DEPTH builds).  Everything that depends on the bit depth is derived from the type at compile time.
+template <typename Pix> struct PixDepth;
+template <> struct PixDepth<uint8_t> { static constexpr int bd = 8; };
+template <> struct PixDepth<uint16_t> { static constexpr int bd = 10; };
+template <typename Pix> struct PixTraits {
+  static constexpr int bd = PixDepth<Pix>::bd;
+  static constexpr int max = (1 << bd) - 1;                           // CLIP_TO_PIXEL (ref: global.h)
+  static constexpr int sao_max = (1 << ((bd < 10 ? bd : 10) - 5)) - 1;  // SAO_ABS_OFFSET_MAX (ref: global.h:230)
+};
+
 // ---------------------------------------------------------------------------------------------- configuration
 // Mirrors the fields of kvz_config / encoder_control_t / encoder_state_t the intra CTU search reads
 // (ref: src/search.c:646-1068, src/search_intra.c, src/intra.c, src/transform.c, src/rdo.c, src/sao.c, src/filter.c).
@@ -89,7 +101,7 @@ struct CtuConfig {
   int32_t cu_split_termination;     // 0 = zero (KVZ_CU_SPLIT_TERMINATION_ZERO), 1 = off
   int32_t intra_rdo_et, combine_intra_cus, intra_chroma_search, full_intra_search;
   int32_t wpp;
-  int32_t pad;
+  int32_t bitdepth;                 // 0 or 8: 8-bit samples, 10: 10-bit samples
   double lambda, lambda_sqrt;       // state->lambda, state->lambda_sqrt
 };
 
@@ -130,17 +142,17 @@ CTU_FN void cbf_set_conditionally(uint16_t *cbf, const uint16_t child[3], int de
 // are what the serial decision code reads all the time: they live in shared memory (CtuS); the pixel and coefficient
 // planes of the level stay in global memory (LcuStore) and are only touched by data-parallel phases.  The source pixels
 // and the border references are the same on every level and live in CtuWork.
-struct LcuStore {
-  uint8_t rec_y[64 * 64], rec_u[32 * 32], rec_v[32 * 32];
+template <typename Pix> struct LcuStore {
+  Pix rec_y[64 * 64], rec_u[32 * 32], rec_v[32 * 32];
   int16_t coeff_y[64 * 64], coeff_u[32 * 32], coeff_v[32 * 32];
 };
-struct LcuLevel {
+template <typename Pix> struct LcuLevel {
   CuRec cu[17 * 17 + 1];
-  uint8_t *rec_y, *rec_u, *rec_v;
+  Pix *rec_y, *rec_u, *rec_v;
   int16_t *coeff_y, *coeff_u, *coeff_v;
 };
-CTU_FN CuRec *cu_at(LcuLevel *L, int x_px, int y_px) { return &L->cu[18 + (x_px >> 2) + (y_px >> 2) * 17]; }   // LCU_GET_CU_AT_PX
-CTU_FN CuRec *cu_top_right(LcuLevel *L) { return &L->cu[17 * 17]; }
+template <typename Pix> CTU_FN CuRec *cu_at(LcuLevel<Pix> *L, int x_px, int y_px) { return &L->cu[18 + (x_px >> 2) + (y_px >> 2) * 17]; }   // LCU_GET_CU_AT_PX
+template <typename Pix> CTU_FN CuRec *cu_top_right(LcuLevel<Pix> *L) { return &L->cu[17 * 17]; }
 
 // z-order offset of a 4-aligned position inside a plane of `width` (ref: xy_to_zorder, src/cu.h:367-402)
 CTU_FN int zorder(int width, int x, int y)
@@ -317,5 +329,7 @@ CTU_FN int scaled_qp(int type, int qp)
   const int mid[14] = { 29, 30, 31, 32, 33, 33, 34, 34, 35, 35, 36, 36, 37, 37 };
   return mid[q - 30];
 }
+// the same with the qp_offset of the bit depth, 6 * (bd - 8) (ref: quant-generic.c:57, 305; rdo.c:672)
+template <typename Pix> CTU_FN int scaled_qp_px(int type, int qp) { return scaled_qp(type, qp) + 6 * (PixDepth<Pix>::bd - 8); }
 
 }  // namespace kvzctu

@@ -11,13 +11,13 @@
 namespace kvzctu {
 
 // Device-resident state of one frame in flight.
-struct FrameDev {
-  const uint8_t *src_y, *src_u, *src_v;     // source planes, stride = width (/2)
-  uint8_t *rec_y, *rec_u, *rec_v;           // reconstruction: search output, then deblocked in place
-  uint8_t *out_y, *out_u, *out_v;           // final picture (after SAO)
-  uint8_t *dbg_y, *dbg_u, *dbg_v;           // optional: the search's reconstruction before deblocking (verification)
-  uint8_t *hor_y, *hor_u, *hor_v;           // hor_buf_search: un-deblocked bottom row of every CTU row
-  uint8_t *ver_y, *ver_u, *ver_v;           // ver_buf_search: un-deblocked right column of every CTU column
+template <typename Pix> struct FrameDevT {
+  const Pix *src_y, *src_u, *src_v;     // source planes, stride = width (/2)
+  Pix *rec_y, *rec_u, *rec_v;           // reconstruction: search output, then deblocked in place
+  Pix *out_y, *out_u, *out_v;           // final picture (after SAO)
+  Pix *dbg_y, *dbg_u, *dbg_v;           // optional: the search's reconstruction before deblocking (verification)
+  Pix *hor_y, *hor_u, *hor_v;           // hor_buf_search: un-deblocked bottom row of every CTU row
+  Pix *ver_y, *ver_u, *ver_v;           // ver_buf_search: un-deblocked right column of every CTU column
   CuRec *cu;                                // per 4x4, stride cu_stride
   int16_t *coeff;                           // per CTU: y[4096] u[1024] v[1024]
   SaoRec *sao;                              // per CTU: [2] luma, chroma
@@ -25,13 +25,14 @@ struct FrameDev {
   int32_t cu_stride;
   int32_t wlcu, hlcu;
 };
+using FrameDev = FrameDevT<uint8_t>;  // (8-bit alias, see CtuWork)
 
 // ------------------------------------------------------------------------------------------------ init_lcu_t
-CTU_FN_NOINLINE void ctu_load(const Ctx &c, const FrameDev *F, int cx, int cy)
+template <typename Pix> CTU_FN_NOINLINE void ctu_load(const CtxT<Pix> &c, const FrameDevT<Pix> *F, int cx, int cy)
 {
   const CtuConfig *cfg = c.cfg;
-  CtuWork *W = c.W;
-  LcuLevel *L0 = &c.S->lv[0];
+  CtuWorkT<Pix> *W = c.W;
+  LcuLevel<Pix> *L0 = &c.S->lv[0];
   const int x = cx * 64, y = cy * 64;
   const int Wd = cfg->width, H = cfg->height;
   // FILL(*lcu, 0) for every level of the work tree (work_tree[depth] = work_tree[0] below only differs in the border
@@ -39,14 +40,14 @@ CTU_FN_NOINLINE void ctu_load(const Ctx &c, const FrameDev *F, int cx, int cy)
   {
     #pragma unroll 1
     for (int d = CTU_TID; d < 5; d += CTU_NT) {
-      LcuLevel *L = &c.S->lv[d];
-      LcuStore *st = &W->store[d];
+      LcuLevel<Pix> *L = &c.S->lv[d];
+      LcuStore<Pix> *st = &W->store[d];
       L->rec_y = st->rec_y; L->rec_u = st->rec_u; L->rec_v = st->rec_v;
       L->coeff_y = st->coeff_y; L->coeff_u = st->coeff_u; L->coeff_v = st->coeff_v;
     }
     uint32_t *p = (uint32_t *)W->store;
     #pragma unroll 1
-    for (int i = CTU_TID; i < (int)(5 * sizeof(LcuStore) / 4); i += CTU_NT) p[i] = 0;
+    for (int i = CTU_TID; i < (int)(5 * sizeof(LcuStore<Pix>) / 4); i += CTU_NT) p[i] = 0;
     uint32_t *q = (uint32_t *)L0->cu;
     #pragma unroll 1
     for (int i = CTU_TID; i < (int)(sizeof(L0->cu) / 4); i += CTU_NT) q[i] = 0;
@@ -126,10 +127,10 @@ CTU_FN_NOINLINE void ctu_load(const Ctx &c, const FrameDev *F, int cx, int cy)
 }
 
 // ------------------------------------------------------------------------------------------------ store
-CTU_FN_NOINLINE void ctu_store(const Ctx &c, const FrameDev *F, int cx, int cy)
+template <typename Pix> CTU_FN_NOINLINE void ctu_store(const CtxT<Pix> &c, const FrameDevT<Pix> *F, int cx, int cy)
 {
   const CtuConfig *cfg = c.cfg;
-  LcuLevel *L0 = &c.S->lv[0];
+  LcuLevel<Pix> *L0 = &c.S->lv[0];
   const int x = cx * 64, y = cy * 64, Wd = cfg->width, H = cfg->height;
   const int x_max = imin(x + 64, Wd) - x, y_max = imin(y + 64, H) - y;
   #pragma unroll 1
@@ -141,7 +142,7 @@ CTU_FN_NOINLINE void ctu_store(const Ctx &c, const FrameDev *F, int cx, int cy)
   for (int e = CTU_TID; e < 64 * 64; e += CTU_NT) {
     const int yy = e >> 6, xx = e & 63;
     if (xx < x_max && yy < y_max) {
-      const uint8_t v = L0->rec_y[e];
+      const Pix v = L0->rec_y[e];
       F->rec_y[(y + yy) * Wd + x + xx] = v;
       if (F->dbg_y) F->dbg_y[(y + yy) * Wd + x + xx] = v;
       if (yy == y_max - 1) F->hor_y[cy * Wd + x + xx] = v;
@@ -152,7 +153,7 @@ CTU_FN_NOINLINE void ctu_store(const Ctx &c, const FrameDev *F, int cx, int cy)
   for (int e = CTU_TID; e < 32 * 32; e += CTU_NT) {
     const int yy = e >> 5, xx = e & 31;
     if (xx < x_max / 2 && yy < y_max / 2) {
-      const uint8_t u = L0->rec_u[e], v = L0->rec_v[e];
+      const Pix u = L0->rec_u[e], v = L0->rec_v[e];
       const int o = (y / 2 + yy) * (Wd / 2) + x / 2 + xx;
       F->rec_u[o] = u; F->rec_v[o] = v;
       if (F->dbg_u) { F->dbg_u[o] = u; F->dbg_v[o] = v; }
@@ -176,10 +177,10 @@ CTU_FN int dbk_tc(int i)
                           4, 5, 5, 6, 6, 7, 8, 9, 10, 11, 13, 14, 16, 18, 20, 22, 24 };
   return t[i];
 }
-CTU_FN const CuRec *fcu(const FrameDev *F, int x, int y) { return &F->cu[(y >> 2) * F->cu_stride + (x >> 2)]; }
+template <typename Pix> CTU_FN const CuRec *fcu(const FrameDevT<Pix> *F, int x, int y) { return &F->cu[(y >> 2) * F->cu_stride + (x >> 2)]; }
 
 // is the left (top) edge of the 8x8 unit at (x, y) a TU or PU boundary (ref: filter.c:194-246)
-CTU_FN bool dbk_edge_wanted(const FrameDev *F, int x, int y, bool hor)
+template <typename Pix> CTU_FN bool dbk_edge_wanted(const FrameDevT<Pix> *F, int x, int y, bool hor)
 {
   const CuRec s = ld_frame_cu(fcu(F, x, y));
   const int tu_w = 64 >> s.tr_depth, cu_w = 64 >> s.depth;
@@ -190,7 +191,7 @@ CTU_FN bool dbk_edge_wanted(const FrameDev *F, int x, int y, bool hor)
 }
 
 // luma part of 4 lines: px -> q0 of line 0; xs across the edge, ys along it (ref: filter.c:95-170, 474-520)
-CTU_FN_NOINLINE void dbk_luma_part(uint8_t *px, int xs, int ys, int beta, int tc)
+template <typename Pix> CTU_FN_NOINLINE void dbk_luma_part(Pix *px, int xs, int ys, int beta, int tc)
 {
   int b[4][8];
   for (int l = 0; l < 4; ++l) for (int i = 0; i < 8; ++i) b[l][i] = CTU_LD_FRAME(&px[l * ys + (i - 4) * xs]);
@@ -205,48 +206,49 @@ CTU_FN_NOINLINE void dbk_luma_part(uint8_t *px, int xs, int ys, int beta, int tc
   const int side = (beta + (beta >> 1)) >> 3;
   for (int l = 0; l < 4; ++l) {
     const int m0 = b[l][0], m1 = b[l][1], m2 = b[l][2], m3 = b[l][3], m4 = b[l][4], m5 = b[l][5], m6 = b[l][6], m7 = b[l][7];
-    uint8_t *row = px + l * ys;
+    Pix *row = px + l * ys;
     if (strong) {
-      row[-3 * xs] = (uint8_t)iclip(m1 - 2 * tc, m1 + 2 * tc, (2 * m0 + 3 * m1 + m2 + m3 + m4 + 4) >> 3);
-      row[-2 * xs] = (uint8_t)iclip(m2 - 2 * tc, m2 + 2 * tc, (m1 + m2 + m3 + m4 + 2) >> 2);
-      row[-1 * xs] = (uint8_t)iclip(m3 - 2 * tc, m3 + 2 * tc, (m1 + 2 * m2 + 2 * m3 + 2 * m4 + m5 + 4) >> 3);
-      row[0] = (uint8_t)iclip(m4 - 2 * tc, m4 + 2 * tc, (m2 + 2 * m3 + 2 * m4 + 2 * m5 + m6 + 4) >> 3);
-      row[xs] = (uint8_t)iclip(m5 - 2 * tc, m5 + 2 * tc, (m3 + m4 + m5 + m6 + 2) >> 2);
-      row[2 * xs] = (uint8_t)iclip(m6 - 2 * tc, m6 + 2 * tc, (m3 + m4 + m5 + 3 * m6 + 2 * m7 + 4) >> 3);
+      row[-3 * xs] = (Pix)iclip(m1 - 2 * tc, m1 + 2 * tc, (2 * m0 + 3 * m1 + m2 + m3 + m4 + 4) >> 3);
+      row[-2 * xs] = (Pix)iclip(m2 - 2 * tc, m2 + 2 * tc, (m1 + m2 + m3 + m4 + 2) >> 2);
+      row[-1 * xs] = (Pix)iclip(m3 - 2 * tc, m3 + 2 * tc, (m1 + 2 * m2 + 2 * m3 + 2 * m4 + m5 + 4) >> 3);
+      row[0] = (Pix)iclip(m4 - 2 * tc, m4 + 2 * tc, (m2 + 2 * m3 + 2 * m4 + 2 * m5 + m6 + 4) >> 3);
+      row[xs] = (Pix)iclip(m5 - 2 * tc, m5 + 2 * tc, (m3 + m4 + m5 + m6 + 2) >> 2);
+      row[2 * xs] = (Pix)iclip(m6 - 2 * tc, m6 + 2 * tc, (m3 + m4 + m5 + 3 * m6 + 2 * m7 + 4) >> 3);
     } else {
       int delta = (9 * (m4 - m3) - 3 * (m5 - m2) + 8) >> 4;
       if (iabs(delta) < tc * 10) {
         delta = iclip(-tc, tc, delta);
-        row[-1 * xs] = (uint8_t)iclip(0, 255, m3 + delta);
-        row[0] = (uint8_t)iclip(0, 255, m4 - delta);
-        if (dp < side) row[-2 * xs] = (uint8_t)iclip(0, 255, m2 + iclip(-(tc >> 1), tc >> 1, (((m1 + m3 + 1) >> 1) - m2 + delta) >> 1));
-        if (dq < side) row[xs] = (uint8_t)iclip(0, 255, m5 + iclip(-(tc >> 1), tc >> 1, (((m6 + m4 + 1) >> 1) - m5 - delta) >> 1));
+        row[-1 * xs] = (Pix)iclip(0, PixTraits<Pix>::max, m3 + delta);
+        row[0] = (Pix)iclip(0, PixTraits<Pix>::max, m4 - delta);
+        if (dp < side) row[-2 * xs] = (Pix)iclip(0, PixTraits<Pix>::max, m2 + iclip(-(tc >> 1), tc >> 1, (((m1 + m3 + 1) >> 1) - m2 + delta) >> 1));
+        if (dq < side) row[xs] = (Pix)iclip(0, PixTraits<Pix>::max, m5 + iclip(-(tc >> 1), tc >> 1, (((m6 + m4 + 1) >> 1) - m5 - delta) >> 1));
       }
     }
   }
 }
-CTU_FN void dbk_chroma_part(uint8_t *px, int xs, int ys, int tc)      // ref: filter.c:175-192
+template <typename Pix> CTU_FN void dbk_chroma_part(Pix *px, int xs, int ys, int tc)      // ref: filter.c:175-192
 {
   for (int l = 0; l < 4; ++l) {
-    uint8_t *s = px + l * ys;
+    Pix *s = px + l * ys;
     const int m2 = CTU_LD_FRAME(&s[-2 * xs]), m3 = CTU_LD_FRAME(&s[-xs]), m4 = CTU_LD_FRAME(&s[0]), m5 = CTU_LD_FRAME(&s[xs]);
     const int delta = iclip(-tc, tc, (((m4 - m3) * 4) + m2 - m5 + 4) >> 3);
-    s[-xs] = (uint8_t)iclip(0, 255, m3 + delta);
-    s[0] = (uint8_t)iclip(0, 255, m4 - delta);
+    s[-xs] = (Pix)iclip(0, PixTraits<Pix>::max, m3 + delta);
+    s[0] = (Pix)iclip(0, PixTraits<Pix>::max, m4 - delta);
   }
 }
 
 // kvz_filter_deblock_lcu on the frame planes; all CUs are intra (boundary strength 2), fixed QP
-CTU_FN_NOINLINE void ctu_deblock(const Ctx &c, const FrameDev *F, int cx, int cy)
+template <typename Pix> CTU_FN_NOINLINE void ctu_deblock(const CtxT<Pix> &c, const FrameDevT<Pix> *F, int cx, int cy)
 {
   const CtuConfig *cfg = c.cfg;
   const int Wd = cfg->width, H = cfg->height, Wc = Wd / 2;
   const int x0 = cx * 64, y0 = cy * 64;
   const int end_x = imin(x0 + 64, Wd), end_y = imin(y0 + 64, H);
   const int qp = cfg->qp;
-  const int beta = dbk_beta(iclip(0, 51, qp + 2 * cfg->deblock_beta));
-  const int tc_l = dbk_tc(iclip(0, 53, qp + 2 + 2 * cfg->deblock_tc));
-  const int tc_c = dbk_tc(iclip(0, 53, scaled_qp(2, qp) + 2 + 2 * cfg->deblock_tc));
+  const int scale = 1 << (PixDepth<Pix>::bd - 8);          // bitdepth_scale (ref: filter.c:373, 590)
+  const int beta = dbk_beta(iclip(0, 51, qp + 2 * cfg->deblock_beta)) * scale;
+  const int tc_l = dbk_tc(iclip(0, 53, qp + 2 + 2 * cfg->deblock_tc)) * scale;
+  const int tc_c = dbk_tc(iclip(0, 53, scaled_qp(2, qp) + 2 + 2 * cfg->deblock_tc)) * scale;
   const int ux_n = (end_x - x0) / 8, uy_n = (end_y - y0) / 8;
   // pass 1: vertical edges of every 8x8 unit: two luma parts per unit, one chroma part where x % 16 == 0
   #pragma unroll 1
@@ -312,20 +314,24 @@ CTU_FN int sao_eo_cat(int a, int b, int cc)
 }
 
 // statistics of the CTU's block of one plane (the reference works on a contiguous copy: same pixels)
-CTU_FN_NOINLINE void sao_stats_plane(const uint8_t *org, const uint8_t *rec, int stride, int bw, int bh, int32_t edge[4][2][5], int32_t band[2][32])
+template <typename Pix> CTU_FN_NOINLINE void sao_stats_plane(const Pix *org, const Pix *rec, int stride, int bw, int bh, int32_t edge[4][2][5], int32_t band[2][32])
 {
+  // bands: the top five bits of the sample (ref: sao.c:273); edge sums: differences rounded to 8-bit precision
+  // (ref: sao-generic.c:66-77)
+  constexpr int band_shift = PixDepth<Pix>::bd - 5, edge_shift = PixDepth<Pix>::bd - 8;
+  constexpr int edge_round = edge_shift ? 1 << (edge_shift - 1) : 0;
   #pragma unroll 1
   for (int e = CTU_TID; e < bw * bh; e += CTU_NT) {
     const int y = e / bw, x = e - y * bw;
     const int cc = CTU_LD_FRAME(&rec[y * stride + x]), d = (int)org[y * stride + x] - cc;
-    CTU_ATOMIC_ADD(&band[0][cc >> 3], d);
-    CTU_ATOMIC_ADD(&band[1][cc >> 3], 1);
+    CTU_ATOMIC_ADD(&band[0][cc >> band_shift], d);
+    CTU_ATOMIC_ADD(&band[1][cc >> band_shift], 1);
     if (x >= 1 && x < bw - 1 && y >= 1 && y < bh - 1) {
       const int ax[4] = { -1, 0, -1, 1 }, ay[4] = { 0, -1, -1, -1 };
       for (int k = 0; k < 4; ++k) {
         const int a = CTU_LD_FRAME(&rec[(y + ay[k]) * stride + x + ax[k]]), b = CTU_LD_FRAME(&rec[(y - ay[k]) * stride + x - ax[k]]);
         const int cat = sao_eo_cat(a, b, cc);
-        CTU_ATOMIC_ADD(&edge[k][0][cat], d);
+        CTU_ATOMIC_ADD(&edge[k][0][cat], (d + edge_round) >> edge_shift);
         CTU_ATOMIC_ADD(&edge[k][1][cat], 1);
       }
     }
@@ -343,26 +349,26 @@ CTU_FN double sao_bits_prefix(const SaoBits &b, bool has_left, bool has_top, int
   m += sao_fbits(b, CTX_SAO_TYPE, type_bin);
   return m;
 }
-CTU_FN double sao_mode_bits_edge(const SaoBits &b, const int *offsets, bool has_top, bool has_left, int buf_cnt)
+template <typename Pix> CTU_FN double sao_mode_bits_edge(const SaoBits &b, const int *offsets, bool has_top, bool has_left, int buf_cnt)
 {
   double m = sao_bits_prefix(b, has_left, has_top, 1);
   m += 1.0;
   for (int bi = 0; bi < buf_cnt; ++bi)
     for (int cat = 1; cat <= 4; ++cat) {
       const int a = iabs(offsets[cat + 5 * bi]);
-      if (a == 0 || a == 7) m += a + 1; else m += a + 2;
+      if (a == 0 || a == PixTraits<Pix>::sao_max) m += a + 1; else m += a + 2;
     }
   m += 2.0;
   return m;
 }
-CTU_FN double sao_mode_bits_band(const SaoBits &b, const int *offsets, bool has_top, bool has_left, int buf_cnt)
+template <typename Pix> CTU_FN double sao_mode_bits_band(const SaoBits &b, const int *offsets, bool has_top, bool has_left, int buf_cnt)
 {
   double m = sao_bits_prefix(b, has_left, has_top, 1);
   m += 1.0;
   for (int bi = 0; bi < buf_cnt; ++bi)
     for (int i = 0; i < 4; ++i) {
       const int a = iabs(offsets[i + 1 + bi * 5]);
-      if (a == 0) m += a + 1; else if (a == 7) m += a + 1 + 1; else m += a + 2 + 1;
+      if (a == 0) m += a + 1; else if (a == PixTraits<Pix>::sao_max) m += a + 1 + 1; else m += a + 2 + 1;
     }
   m += 5.0 * buf_cnt;
   return m;
@@ -379,12 +385,12 @@ CTU_FN int sao_band_ddist(const int32_t bd[2][32], int band_pos, const int *offs
   for (int k = 0; k < 4; ++k) { const int o = offs[k], bi = band_pos + k; if (o != 0 && bi >= 0 && bi < 32) sum += bd[1][bi] * o * o - 2 * o * bd[0][bi]; }
   return sum;
 }
-CTU_FN_NOINLINE int sao_band_offsets(const int32_t bd[2][32], int *offsets /* [4] */, int *band_position)
+template <typename Pix> CTU_FN_NOINLINE int sao_band_offsets(const int32_t bd[2][32], int *offsets /* [4] */, int *band_position)
 {
   int dist[32], temp_offsets[32];
   for (int band = 0; band < 32; ++band) {
     int best_dist = CTU_MAX_INT, offset = 0;
-    if (bd[1][band] != 0) { offset = (bd[0][band] + (bd[1][band] >> 1)) / bd[1][band]; offset = iclip(-7, 7, offset); }
+    if (bd[1][band] != 0) { offset = (bd[0][band] + (bd[1][band] >> 1)) / bd[1][band]; offset = iclip(-PixTraits<Pix>::sao_max, PixTraits<Pix>::sao_max, offset); }
     dist[band] = offset == 0 ? 0 : CTU_MAX_INT;
     temp_offsets[band] = 0;
     while (offset != 0) {
@@ -405,7 +411,7 @@ CTU_FN_NOINLINE int sao_band_offsets(const int32_t bd[2][32], int *offsets /* [4
 }
 
 // sao_search_best_mode for one component group (luma: planes {0}, chroma: planes {1, 2}).  Leader only.
-CTU_FN_NOINLINE void sao_search_best_mode(const Ctx &c, const SaoStats *st, int first_plane, int buf_cnt, SaoRec *out, const SaoRec *top, const SaoRec *left, int32_t merge_cost[3])
+template <typename Pix> CTU_FN_NOINLINE void sao_search_best_mode(const CtxT<Pix> &c, const SaoStats *st, int first_plane, int buf_cnt, SaoRec *out, const SaoRec *top, const SaoRec *left, int32_t merge_cost[3])
 {
   const CtuConfig *cfg = c.cfg;
   const SaoBits sb = { &c.S->tb, c.S->cabac0.ctx };
@@ -423,7 +429,7 @@ CTU_FN_NOINLINE void sao_search_best_mode(const Ctx &c, const SaoStats *st, int 
         for (int cat = 1; cat <= 4; ++cat) {
           const int cat_sum = s[0][cat], cat_cnt = s[1][cat];
           int offset = 0;
-          if (cat_cnt != 0) { offset = (cat_sum + (cat_cnt >> 1)) / cat_cnt; offset = iclip(-7, 7, offset); }
+          if (cat_cnt != 0) { offset = (cat_sum + (cat_cnt >> 1)) / cat_cnt; offset = iclip(-PixTraits<Pix>::sao_max, PixTraits<Pix>::sao_max, offset); }
           if (cat <= 2 && offset < 0) offset = 0;
           if (cat >= 3 && offset > 0) offset = 0;
           eo[cat + 5 * i] = offset;
@@ -431,13 +437,13 @@ CTU_FN_NOINLINE void sao_search_best_mode(const Ctx &c, const SaoStats *st, int 
         }
       }
       {
-        const float mode_bits = (float)sao_mode_bits_edge(sb, eo, top != NULL, left != NULL, buf_cnt);
+        const float mode_bits = (float)sao_mode_bits_edge<Pix>(sb, eo, top != NULL, left != NULL, buf_cnt);
         sum_dd += (int)((double)mode_bits * lambda + 0.5);
       }
       eo[0] = 0; eo[5] = 0;
       if (sum_dd < edge.ddistortion) { edge.eo_class = cls; edge.ddistortion = sum_dd; for (int i = 0; i < 10; ++i) edge.offsets[i] = eo[i]; }
     }
-    const float mode_bits = (float)sao_mode_bits_edge(sb, edge.offsets, top != NULL, left != NULL, buf_cnt);
+    const float mode_bits = (float)sao_mode_bits_edge<Pix>(sb, edge.offsets, top != NULL, left != NULL, buf_cnt);
     int dd = (int)(mode_bits * lambda + 0.5);
     for (int i = 0; i < buf_cnt; ++i) dd += sao_edge_ddist(st->edge[first_plane + i][edge.eo_class], &edge.offsets[5 * i]);
     edge.ddistortion = dd;
@@ -447,11 +453,11 @@ CTU_FN_NOINLINE void sao_search_best_mode(const Ctx &c, const SaoStats *st, int 
     int temp_offsets[10];
     for (int i = 0; i < 10; ++i) temp_offsets[i] = 0;
     int dd = 0;
-    for (int i = 0; i < buf_cnt; ++i) dd += sao_band_offsets(st->band[first_plane + i], &temp_offsets[1 + 5 * i], &band.band_position[i]);
-    const float temp_rate = (float)sao_mode_bits_band(sb, temp_offsets, top != NULL, left != NULL, buf_cnt);
+    for (int i = 0; i < buf_cnt; ++i) dd += sao_band_offsets<Pix>(st->band[first_plane + i], &temp_offsets[1 + 5 * i], &band.band_position[i]);
+    const float temp_rate = (float)sao_mode_bits_band<Pix>(sb, temp_offsets, top != NULL, left != NULL, buf_cnt);
     dd += (int)((double)temp_rate * lambda + 0.5);
     if (dd < band.ddistortion) { band.ddistortion = dd; for (int i = 0; i < buf_cnt * 5; ++i) band.offsets[i] = temp_offsets[i]; }
-    const float mode_bits = (float)sao_mode_bits_band(sb, band.offsets, top != NULL, left != NULL, buf_cnt);
+    const float mode_bits = (float)sao_mode_bits_band<Pix>(sb, band.offsets, top != NULL, left != NULL, buf_cnt);
     int d2 = (int)(mode_bits * lambda + 0.5);
     for (int i = 0; i < buf_cnt; ++i) d2 += sao_band_ddist(st->band[first_plane + i], band.band_position[i], &band.offsets[1 + 5 * i]);
     band.ddistortion = d2;
@@ -479,7 +485,7 @@ CTU_FN_NOINLINE void sao_search_best_mode(const Ctx &c, const SaoStats *st, int 
 }
 
 // kvz_sao_search_lcu; `st` is scratch for the statistics (global or shared)
-CTU_FN_NOINLINE void ctu_sao_search(const Ctx &c, const FrameDev *F, SaoStats *st, int cx, int cy)
+template <typename Pix> CTU_FN_NOINLINE void ctu_sao_search(const CtxT<Pix> &c, const FrameDevT<Pix> *F, SaoStats *st, int cx, int cy)
 {
   const CtuConfig *cfg = c.cfg;
   const int Wd = cfg->width, H = cfg->height;
@@ -531,13 +537,13 @@ CTU_FN void enc_bin(const SmTables *T, uint8_t *ctx, int off, int val)
 
 // All records and coefficients come from level 0 of the work tree: after the search it holds the CTU's decisions (the
 // same values ctu_store wrote to the frame) and the border records of the left / above CTUs (ctu_load).
-struct EncTrack { const Ctx *c; LcuLevel *L0; int x0, y0; CabacState *cs; };
-CTU_FN const CuRec *tcu(const EncTrack &e, int x, int y) { return cu_at(e.L0, x - e.x0, y - e.y0); }
+template <typename Pix> struct EncTrack { const CtxT<Pix> *c; LcuLevel<Pix> *L0; int x0, y0; CabacState *cs; };
+template <typename Pix> CTU_FN const CuRec *tcu(const EncTrack<Pix> &e, int x, int y) { return cu_at(e.L0, x - e.x0, y - e.y0); }
 
 // encode_transform_coeff + encode_transform_unit (ref: encode_coding_tree.c:117-319), context-coded bins only
-CTU_FN_NOINLINE void enc_transform_leaf(const EncTrack &e, int x, int y, int depth, int tr_depth, int parent_u, int parent_v)
+template <typename Pix> CTU_FN_NOINLINE void enc_transform_leaf(const EncTrack<Pix> &e, int x, int y, int depth, int tr_depth, int parent_u, int parent_v)
 {
-  const Ctx &c = *e.c;
+  const CtxT<Pix> &c = *e.c;
   const CuRec *cur_pu = tcu(e, x, y);
   const CuRec *cur_cu = tcu(e, x & ~7, y & ~7);
   const int cb_y = cbf_is_set(cur_pu->cbf, depth, 0), cb_u = cbf_is_set(cur_cu->cbf, depth, 1), cb_v = cbf_is_set(cur_cu->cbf, depth, 2);
@@ -567,10 +573,10 @@ CTU_FN_NOINLINE void enc_transform_leaf(const EncTrack &e, int x, int y, int dep
     if (cu_v) coeff_cost_serial(&c.S->tb, &c.S->tb, c.cfg, e.cs, e.L0->coeff_v + zi, ilog2(width_c), 2, scan, 0);
   }
 }
-CTU_FN void enc_transform_tree(const EncTrack &e, int x, int y, int depth)
+template <typename Pix> CTU_FN void enc_transform_tree(const EncTrack<Pix> &e, int x, int y, int depth)
 {
   // root of the CU's transform tree: tr_depth 0
-  const Ctx &c = *e.c;
+  const CtxT<Pix> &c = *e.c;
   const CuRec *cur_cu = tcu(e, x & ~7, y & ~7);
   const int split = cur_cu->tr_depth > depth;
   if (!split) { enc_transform_leaf(e, x, y, depth, 0, 0, 0); return; }
@@ -582,9 +588,9 @@ CTU_FN void enc_transform_tree(const EncTrack &e, int x, int y, int depth)
 }
 
 // one coding unit (no further split): part mode, intra modes, transform tree
-CTU_FN_NOINLINE void enc_coding_unit(const EncTrack &e, int x, int y, int depth)
+template <typename Pix> CTU_FN_NOINLINE void enc_coding_unit(const EncTrack<Pix> &e, int x, int y, int depth)
 {
-  const Ctx &c = *e.c;
+  const CtxT<Pix> &c = *e.c;
   const CuRec *cur_cu = tcu(e, x, y);
   const int cu_width = 64 >> depth;
   if (depth == 3) enc_bin(&c.S->tb, e.cs->ctx, CTX_PART_SIZE, cur_cu->part_size == SIZE_2Nx2N ? 1 : 0);
@@ -608,9 +614,9 @@ CTU_FN_NOINLINE void enc_coding_unit(const EncTrack &e, int x, int y, int depth)
 }
 
 // kvz_encode_coding_tree: explicit traversal of the CU quadtree in coding order
-CTU_FN_NOINLINE void enc_coding_tree(const EncTrack &e, int x0, int y0)
+template <typename Pix> CTU_FN_NOINLINE void enc_coding_tree(const EncTrack<Pix> &e, int x0, int y0)
 {
-  const Ctx &c = *e.c;
+  const CtxT<Pix> &c = *e.c;
   const int Wd = c.cfg->width, H = c.cfg->height;
   // depth-first with a small stack of (x, y, depth)
   int sx[16], sy[16], sd[16], sp = 0;
@@ -646,7 +652,7 @@ CTU_FN_NOINLINE void enc_coding_tree(const EncTrack &e, int x0, int y0)
 
 // The CTU's effect on the real coder's models; afterwards the row's state is published (and handed to the next row
 // after the second CTU: WPP, encoderstate.c:759-771).  Leader only inside.
-CTU_FN_NOINLINE void ctu_track_models(const Ctx &c, const FrameDev *F, int cx, int cy)
+template <typename Pix> CTU_FN_NOINLINE void ctu_track_models(const CtxT<Pix> &c, const FrameDevT<Pix> *F, int cx, int cy)
 {
   CTU_LEADER {
     CabacState cs = c.S->cabac0;
@@ -660,7 +666,7 @@ CTU_FN_NOINLINE void ctu_track_models(const Ctx &c, const FrameDev *F, int cx, i
         enc_bin(&c.S->tb, cs.ctx, CTX_SAO_TYPE, sc->type != 0);
       }
     }
-    EncTrack e = { &c, &c.S->lv[0], cx * 64, cy * 64, &cs };
+    EncTrack<Pix> e = { &c, &c.S->lv[0], cx * 64, cy * 64, &cs };
     enc_coding_tree(e, cx * 64, cy * 64);
     cs.update = 0;
     F->row_ctx[cy] = cs;
@@ -670,7 +676,7 @@ CTU_FN_NOINLINE void ctu_track_models(const Ctx &c, const FrameDev *F, int cx, i
 }
 
 // ------------------------------------------------------------------------------------------------ whole CTU job
-CTU_FN void ctu_job(const Ctx &c, const FrameDev *F, SaoStats *sao_scratch, int cx, int cy)
+template <typename Pix> CTU_FN void ctu_job(const CtxT<Pix> &c, const FrameDevT<Pix> *F, SaoStats *sao_scratch, int cx, int cy)
 {
   { PROF_T0(PR_LOAD); ctu_load(c, F, cx, cy); PROF_ADD(c.S, PR_LOAD); }
   { PROF_T0(PR_SEARCH); search_ctu(c, cx * 64, cy * 64); PROF_ADD(c.S, PR_SEARCH); }
@@ -690,15 +696,15 @@ CTU_FN void ctu_job(const Ctx &c, const FrameDev *F, SaoStats *sao_scratch, int 
 // Final picture of one CTU area from the deblocked planes (kvz_sao_reconstruct + sao_reconstruct_color semantics,
 // sao.c:302-361, sao-generic.c:84-124): neighbours come from the deblocked picture, samples whose neighbour lies
 // outside the picture keep their value.
-CTU_FN_NOINLINE void ctu_sao_apply(const CtuConfig *cfg, const FrameDev *F, int cx, int cy)
+template <typename Pix> CTU_FN_NOINLINE void ctu_sao_apply(const CtuConfig *cfg, const FrameDevT<Pix> *F, int cx, int cy)
 {
   const int Wd = cfg->width, H = cfg->height;
   const SaoRec *sl = &F->sao[2 * (cy * F->wlcu + cx)], *sc = sl + 1;
   for (int plane = 0; plane < 3; ++plane) {
     const int sh = plane ? 1 : 0;
     const int pw = Wd >> sh, ph = H >> sh;
-    const uint8_t *in = plane == 0 ? F->rec_y : (plane == 1 ? F->rec_u : F->rec_v);
-    uint8_t *out = plane == 0 ? F->out_y : (plane == 1 ? F->out_u : F->out_v);
+    const Pix *in = plane == 0 ? F->rec_y : (plane == 1 ? F->rec_u : F->rec_v);
+    Pix *out = plane == 0 ? F->out_y : (plane == 1 ? F->out_u : F->out_v);
     const SaoRec *s = plane == 0 ? sl : sc;
     const int x0 = (cx * 64) >> sh, y0 = (cy * 64) >> sh;
     const int bw = imin(64 >> sh, pw - x0), bh = imin(64 >> sh, ph - y0);
@@ -711,17 +717,17 @@ CTU_FN_NOINLINE void ctu_sao_apply(const CtuConfig *cfg, const FrameDev *F, int 
       const int cc = in[(size_t)y * pw + x];
       int v = cc;
       if (type == 1) {
-        const int k = (cc >> 3) - s->band_position[plane == 2 ? 1 : 0];
-        if (k >= 0 && k <= 3) v = iclip(0, 255, cc + s->offsets[k + 1 + ov]);
+        const int k = (cc >> (PixDepth<Pix>::bd - 5)) - s->band_position[plane == 2 ? 1 : 0];
+        if (k >= 0 && k <= 3) v = iclip(0, PixTraits<Pix>::max, cc + s->offsets[k + 1 + ov]);
       } else if (type == 2) {
         const int dx = ax[s->eo_class], dy = ay[s->eo_class];
         const int xa = x + dx, ya = y + dy, xb = x - dx, yb = y - dy;
         if (xa >= 0 && xa < pw && xb >= 0 && xb < pw && ya >= 0 && ya < ph && yb >= 0 && yb < ph) {
           const int cat = sao_eo_cat(in[(size_t)ya * pw + xa], in[(size_t)yb * pw + xb], cc);
-          v = iclip(0, 255, cc + s->offsets[cat + ov]);
+          v = iclip(0, PixTraits<Pix>::max, cc + s->offsets[cat + ov]);
         }
       }
-      out[(size_t)y * pw + x] = (uint8_t)v;
+      out[(size_t)y * pw + x] = (Pix)v;
     }
   }
 }

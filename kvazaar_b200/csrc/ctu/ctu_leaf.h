@@ -1,7 +1,7 @@
 // ctu_leaf.h -- block-level operations of the CTU search driver, written for the execution model of ctu_common.h
 // (every function is called by all threads of the CTA unless it says "leader only" / "team").
 //
-// Reference semantics restated here (8-bit, 4:2:0, flat scaling lists):
+// Reference semantics restated here (8- and 10-bit, 4:2:0, flat scaling lists):
 //   intra references     src/intra.c:305-559 (kvz_intra_build_reference_any / _inner), :176-204 (smoothing)
 //   intra prediction     src/intra.c:252-302 + strategies/generic/intra-generic.c:49-241
 //   SATD / SAD           strategies/generic/picture-generic.c:117-340, 475-501
@@ -27,20 +27,23 @@ namespace kvzctu {
 // written back instead of computed a second time.  Luma: unit (candidate * alternatives + alternative), the alternatives
 // being transform / transform skip of a 4x4 unit; chroma: unit (candidate).  Units of the CU's size, back to back.
 #define CTU_RDO_CANDS 6             // search_intra_rdo: at most 3 rough-search modes (2 above depth 4) and the 3 MPMs
-struct CandStore {
-  uint8_t rec_y[CTU_RDO_CANDS * 1024], rec_c[2][CTU_RDO_CANDS * 256];
+template <typename Pix> struct CandStore {
+  Pix rec_y[CTU_RDO_CANDS * 1024], rec_c[2][CTU_RDO_CANDS * 256];
   int16_t q_y[CTU_RDO_CANDS * 1024], q_c[2][CTU_RDO_CANDS * 256];
 };
-struct CtuWork {                    // per resident CTU, global memory (L2 resident)
-  LcuStore store[5];
-  CandStore cand;
-  uint8_t src_y[64 * 64], src_u[32 * 32], src_v[32 * 32];       // lcu->ref
+template <typename Pix> struct CtuWorkT {                    // per resident CTU, global memory (L2 resident)
+  LcuStore<Pix> store[5];
+  CandStore<Pix> cand;
+  Pix src_y[64 * 64], src_u[32 * 32], src_v[32 * 32];       // lcu->ref
   // border references from the neighbouring CTUs, index 0 = top-left corner sample (lcu->top_ref / left_ref)
-  uint8_t top_y[100], top_u[52], top_v[52], left_y[100], left_u[52], left_v[52];
+  Pix top_y[100], top_u[52], top_v[52], left_y[100], left_u[52], left_v[52];
 };
+// The 8-bit instantiations of the types the driver's host code names (CtuWork, CtuS, FrameDev, Ctx) keep their plain
+// names as aliases: 8-bit code written before the sample type became a parameter compiles unchanged.
+using CtuWork = CtuWorkT<uint8_t>;
 
-struct IntraRefs {                  // kvz_intra_references: index 0 = corner, 1..2w along the edge
-  uint8_t top[68], left[68], ftop[68], fleft[68];
+template <typename Pix> struct IntraRefs {                  // kvz_intra_references: index 0 = corner, 1..2w along the edge
+  Pix top[68], left[68], ftop[68], fleft[68];
   int32_t dc;                       // DC value of the unfiltered references (modes 1)
   int32_t pad;
 };
@@ -103,7 +106,7 @@ CTU_FN void sm_tables_load(SmTables *d, const CtuTables *g)
 }
 
 // Scratch of one transform-unit evaluation, carved out of the team's part of the arena for nn = n*n coefficients.
-struct TuFixed {
+template <typename Pix> struct TuFixed {
   double prep_c0[16], prep_sig0[16], prep_sig1[16];
   int32_t prep_ld[16], prep_ctx_sig[16];
   int32_t last_x_bits[12], last_y_bits[12];
@@ -113,21 +116,21 @@ struct TuFixed {
   uint32_t cg_mask[2];              // coefficient groups (raster) with a level != 0, of the unit's final levels
   uint32_t ts_mask[2];
   // transform skip decision (kvz_quantize_residual_trskip): both alternatives of a 4x4 luma unit
-  uint8_t ts_rec[2][16];
+  Pix ts_rec[2][16];
   int16_t ts_coeff[2][16];
   int32_t ts_has[2], ts_ssd[2];
   int32_t ts_pick, pad;
 };
-static_assert(sizeof(TuFixed) % 8 == 0, "TuFixed alignment");
-struct TuS {
+static_assert(sizeof(TuFixed<uint8_t>) % 8 == 0 && sizeof(TuFixed<uint16_t>) % 8 == 0, "TuFixed alignment");
+template <typename Pix> struct TuS {
   unsigned char *base;
   int nn, ncg;
   // doubles
   CTU_MFN double *cost_coeff() const { return (double *)base; }
   CTU_MFN double *cg_sig_cost() const { return (double *)base + nn; }
-  CTU_MFN TuFixed *fx() const { return (TuFixed *)((double *)base + nn + ncg); }
+  CTU_MFN TuFixed<Pix> *fx() const { return (TuFixed<Pix> *)((double *)base + nn + ncg); }
   // 32-bit: kvz_sh_rates_t (rdo.h:49-58); d (delta_u of kvz_quant's sign hiding) shares inc: never both
-  CTU_MFN int32_t *i32() const { return (int32_t *)(base + 8 * (nn + ncg) + sizeof(TuFixed)); }
+  CTU_MFN int32_t *i32() const { return (int32_t *)(base + 8 * (nn + ncg) + sizeof(TuFixed<Pix>)); }
   CTU_MFN int32_t *inc() const { return i32(); }
   CTU_MFN int32_t *dec() const { return i32() + nn; }
   CTU_MFN int32_t *sig_inc() const { return i32() + 2 * nn; }
@@ -145,29 +148,31 @@ struct TuS {
   // bytes
   CTU_MFN uint8_t *u8() const { return (uint8_t *)(i16() + 4 * nn + ncg + (ncg & 1)); }
   CTU_MFN uint8_t *sig_code() const { return u8(); }
-  CTU_MFN uint8_t *pred() const { return u8() + nn; }
-  CTU_MFN uint8_t *rec() const { return u8() + 2 * nn; }
+  CTU_MFN Pix *pred() const { return (Pix *)(u8() + nn); }
+  CTU_MFN Pix *rec() const { return pred() + nn; }
 };
-CTU_FN int tu_scratch_bytes(int nn)
+template <typename Pix> CTU_FN int tu_scratch_bytes(int nn)
 {
   const int ncg = nn >= 16 ? nn / 16 : 1;
-  const int b = 8 * (nn + ncg) + (int)sizeof(TuFixed) + 4 * (4 * nn + 2 * ncg) + 2 * (4 * nn + ncg + (ncg & 1)) + 3 * nn;
+  const int b = 8 * (nn + ncg) + (int)sizeof(TuFixed<Pix>) + 4 * (4 * nn + 2 * ncg) + 2 * (4 * nn + ncg + (ncg & 1)) + nn + 2 * nn * (int)sizeof(Pix);
   return (b + 15) & ~15;
 }
-CTU_FN TuS tu_scratch(unsigned char *arena, int nn, int slot)
+template <typename Pix> CTU_FN TuS<Pix> tu_scratch(unsigned char *arena, int nn, int slot)
 {
-  TuS t;
+  TuS<Pix> t;
   t.nn = nn; t.ncg = nn >= 16 ? nn / 16 : 1;
-  t.base = arena + (size_t)slot * tu_scratch_bytes(nn);
+  t.base = arena + (size_t)slot * tu_scratch_bytes<Pix>(nn);
   return t;
 }
-#define CTU_ARENA_BYTES 40960      // one 32x32 unit, or four units of up to 16x16 side by side
+// One 32x32 unit, or four units of up to 16x16 side by side.  With 16-bit samples four 16x16 units need 42 176 bytes:
+// the arena keeps its size (three CTAs per SM) and for_tu_tasks runs such units one after another on the whole CTA.
+#define CTU_ARENA_BYTES 40960
 
 // ------------------------------------------------------------------------------------------------ pixel planes
-struct Plane { uint8_t *rec; const uint8_t *src; const uint8_t *top; const uint8_t *left; int16_t *coeff; int lw; };
-CTU_FN Plane plane_of(CtuWork *W, LcuLevel *L, int color)
+template <typename Pix> struct Plane { Pix *rec; const Pix *src; const Pix *top; const Pix *left; int16_t *coeff; int lw; };
+template <typename Pix> CTU_FN Plane<Pix> plane_of(CtuWorkT<Pix> *W, LcuLevel<Pix> *L, int color)
 {
-  Plane p;
+  Plane<Pix> p;
   if (color == 0) { p.rec = L->rec_y; p.src = W->src_y; p.top = W->top_y; p.left = W->left_y; p.coeff = L->coeff_y; p.lw = 64; }
   else if (color == 1) { p.rec = L->rec_u; p.src = W->src_u; p.top = W->top_u; p.left = W->left_u; p.coeff = L->coeff_u; p.lw = 32; }
   else { p.rec = L->rec_v; p.src = W->src_v; p.top = W->top_v; p.left = W->left_v; p.coeff = L->coeff_v; p.lw = 32; }
@@ -179,10 +184,11 @@ CTU_FN Plane plane_of(CtuWork *W, LcuLevel *L, int color)
 // coordinates), into r[colour], followed by the [1 2 1] smoothing (done eagerly: the reference's lazy flag only saves
 // time; chroma never reads it) and the DC sum.  log2w[colour]: the block sizes.  One pass over all colours: the border
 // reads of the three planes overlap instead of queueing behind each other.
-CTU_FN_NOINLINE void build_refs_multi(const SmTables *T, const CtuConfig *cfg, CtuWork *W, LcuLevel *L, const int log2w[3], int mask, int x, int y, IntraRefs *r)
+template <typename Pix> CTU_FN_NOINLINE void build_refs_multi(const SmTables *T, const CtuConfig *cfg, CtuWorkT<Pix> *W, LcuLevel<Pix> *L, const int log2w[3], int mask, int x, int y, IntraRefs<Pix> *r)
 {
   const int lx = x & 63, ly = y & 63;
   const bool has_left = x > 0, has_top = y > 0, inner = has_left && has_top;
+  const int mid = 1 << (PixDepth<Pix>::bd - 1);       // value of unavailable references (ref: intra.c:319)
   int n_of[3], start[4];
   start[0] = 0;
   for (int col = 0; col < 3; ++col) { n_of[col] = ((mask >> col) & 1) ? 2 * (1 << log2w[col]) + 1 : 0; start[col + 1] = start[col] + 2 * n_of[col]; }
@@ -191,7 +197,7 @@ CTU_FN_NOINLINE void build_refs_multi(const SmTables *T, const CtuConfig *cfg, C
     const int color = it >= start[2] ? 2 : (it >= start[1] ? 1 : 0);
     const int i = it - start[color], n = n_of[color], w = (n - 1) >> 1;
     const int is_c = color != 0;
-    const Plane P = plane_of(W, L, color);
+    const Plane<Pix> P = plane_of(W, L, color);
     const int px = lx >> is_c, py = ly >> is_c, lw = P.lw;
     int al = 0, at = 0;
     if (has_left) { al = T->ref_left[ly >> 2][lx >> 2] >> is_c; al = imin(al, 2 * w); al = imin(al, (cfg->height - y) >> is_c); }
@@ -207,17 +213,17 @@ CTU_FN_NOINLINE void build_refs_multi(const SmTables *T, const CtuConfig *cfg, C
     int v;
     if (e == 0) {
       if (inner) v = px ? CTU_TOP_BORDER(-1) : CTU_LEFT_BORDER(-1);
-      else v = has_left ? CTU_LEFT_BORDER(0) : (has_top ? CTU_TOP_BORDER(0) : 128);      // "copy reference clockwise": left[1]
+      else v = has_left ? CTU_LEFT_BORDER(0) : (has_top ? CTU_TOP_BORDER(0) : mid);      // "copy reference clockwise": left[1]
     } else if (!is_top) {
       if (has_left) v = CTU_LEFT_BORDER(imin(e - 1, nl - 1));
-      else v = has_top ? CTU_TOP_BORDER(0) : 128;
+      else v = has_top ? CTU_TOP_BORDER(0) : mid;
     } else {
       if (has_top) v = CTU_TOP_BORDER(imin(e - 1, ntp - 1));
-      else v = has_left ? CTU_LEFT_BORDER(0) : 128;
+      else v = has_left ? CTU_LEFT_BORDER(0) : mid;
     }
 #undef CTU_TOP_BORDER
 #undef CTU_LEFT_BORDER
-    (is_top ? r[color].top : r[color].left)[e] = (uint8_t)v;
+    (is_top ? r[color].top : r[color].left)[e] = (Pix)v;
   }
   CTU_SYNC();
   // smoothing of the luma references; one thread per colour sums the DC
@@ -236,29 +242,29 @@ CTU_FN_NOINLINE void build_refs_multi(const SmTables *T, const CtuConfig *cfg, C
     }
     const bool is_top = i >= n0;
     const int e = is_top ? i - n0 : i;
-    const uint8_t *p = is_top ? r[0].top : r[0].left;
+    const Pix *p = is_top ? r[0].top : r[0].left;
     int v;
     if (e == 0) v = (r[0].left[1] + 2 * r[0].left[0] + r[0].top[1] + 2) >> 2;
     else if (e == n0 - 1) v = p[e];
     else v = (p[e - 1] + 2 * p[e] + p[e + 1] + 2) >> 2;
-    (is_top ? r[0].ftop : r[0].fleft)[e] = (uint8_t)v;
+    (is_top ? r[0].ftop : r[0].fleft)[e] = (Pix)v;
   }
   CTU_SYNC();
 }
-CTU_FN void build_refs(const SmTables *T, const CtuConfig *cfg, CtuWork *W, LcuLevel *L, int log2w, int color, int x, int y, IntraRefs *r)
+template <typename Pix> CTU_FN void build_refs(const SmTables *T, const CtuConfig *cfg, CtuWorkT<Pix> *W, LcuLevel<Pix> *L, int log2w, int color, int x, int y, IntraRefs<Pix> *r)
 {
   int l[3] = { log2w, log2w, log2w };
   build_refs_multi(T, cfg, W, L, l, 1 << color, x, y, r - color);
 }
 
 // ------------------------------------------------------------------------------------------------ intra prediction
-CTU_FN int ang_ref(const uint8_t *rmain, const uint8_t *rside, int idx, int inv)
+template <typename Pix> CTU_FN int ang_ref(const Pix *rmain, const Pix *rside, int idx, int inv)
 {
   if (idx >= -1) return rmain[idx + 1];
   const int k = -idx - 1;
   return rside[(128 + k * inv) >> 8];
 }
-CTU_FN int angular_px(int mode, const uint8_t *top, const uint8_t *left, int ox, int oy)
+template <typename Pix> CTU_FN int angular_px(int mode, const Pix *top, const Pix *left, int ox, int oy)
 {
   const int disp_tab[9] = { 0, 2, 5, 9, 13, 17, 21, 26, 32 };
   const int inv_tab[9] = { 0, 4096, 1638, 910, 630, 482, 390, 315, 256 };
@@ -266,8 +272,8 @@ CTU_FN int angular_px(int mode, const uint8_t *top, const uint8_t *left, int ox,
   const int mdisp = vertical ? mode - 26 : 10 - mode;
   const int adisp = iabs(mdisp);
   const int sdisp = mdisp < 0 ? -disp_tab[adisp] : disp_tab[adisp];
-  const uint8_t *rmain = vertical ? top : left;
-  const uint8_t *rside = vertical ? left : top;
+  const Pix *rmain = vertical ? top : left;
+  const Pix *rside = vertical ? left : top;
   const int x = vertical ? ox : oy, y = vertical ? oy : ox;
   if (sdisp == 0) return rmain[x + 1];
   const int pos = (y + 1) * sdisp;
@@ -286,10 +292,10 @@ CTU_FN bool intra_uses_filtered(int log2w, int mode, int color)
   return imin(iabs(mode - 26), iabs(mode - 10)) > thres;
 }
 // kvz_intra_predict for one sample (filter_boundary is always true: no lossless / implicit RDPCM)
-CTU_FN int intra_predict_px(const IntraRefs *r, int log2w, int mode, int color, int x, int y)
+template <typename Pix> CTU_FN int intra_predict_px(const IntraRefs<Pix> *r, int log2w, int mode, int color, int x, int y)
 {
   const bool f = intra_uses_filtered(log2w, mode, color);
-  const uint8_t *t = f ? r->ftop : r->top, *l = f ? r->fleft : r->left;
+  const Pix *t = f ? r->ftop : r->top, *l = f ? r->fleft : r->left;
   const int w = 1 << log2w;
   if (mode == 0) {
     const int hor = (w - 1 - x) * l[y + 1] + (x + 1) * t[w + 1];
@@ -307,19 +313,19 @@ CTU_FN int intra_predict_px(const IntraRefs *r, int log2w, int mode, int color, 
   }
   int v = angular_px(mode, t, l, x, y);
   if (color == 0 && log2w < 5) {
-    if (mode == 10 && y == 0) v = iclip(0, 255, v + ((t[x + 1] - t[0]) >> 1));
-    else if (mode == 26 && x == 0) v = iclip(0, 255, v + ((l[y + 1] - l[0]) >> 1));
+    if (mode == 10 && y == 0) v = iclip(0, PixTraits<Pix>::max, v + ((t[x + 1] - t[0]) >> 1));
+    else if (mode == 26 && x == 0) v = iclip(0, PixTraits<Pix>::max, v + ((l[y + 1] - l[0]) >> 1));
   }
   return v;
 }
 // prediction of a whole block into dst (row stride dst_stride)
-CTU_FN_NOINLINE void predict_block(const IntraRefs *r, int log2w, int mode, int color, uint8_t *dst, int dst_stride)
+template <typename Pix> CTU_FN_NOINLINE void predict_block(const IntraRefs<Pix> *r, int log2w, int mode, int color, Pix *dst, int dst_stride)
 {
   const int w = 1 << log2w;
   #pragma unroll 1
   for (int e = CTU_TID; e < w * w; e += CTU_NT) {
     const int y = e >> log2w, x = e & (w - 1);
-    dst[y * dst_stride + x] = (uint8_t)intra_predict_px(r, log2w, mode, color, x, y);
+    dst[y * dst_stride + x] = (Pix)intra_predict_px(r, log2w, mode, color, x, y);
   }
   CTU_SYNC();
 }
@@ -368,8 +374,8 @@ CTU_FN int hadamard8_abs_sum(int d[64])
 // ref_main[idx + 1] holds (intra-generic.c:86-122) -- the main edge for idx >= -1, the projected side edge below --
 // so that a sample is one branch-free two-tap interpolation.  Horizontal modes are evaluated transposed (main = left,
 // block and source transposed): the SATD / SAD of a block and of its transpose are the same.
-struct RoughExt { uint8_t e[33][104]; };      // [mode - 2][idx + w], idx in [-w, 2w + 1]
-static_assert(sizeof(RoughExt) <= CTU_ARENA_BYTES, "rough-search scratch lives in the arena");
+template <typename Pix> struct RoughExt { Pix e[33][104]; };      // [mode - 2][idx + w], idx in [-w, 2w + 1]
+static_assert(sizeof(RoughExt<uint16_t>) <= CTU_ARENA_BYTES, "rough-search scratch lives in the arena");
 
 CTU_FN void ang_params(int mode, bool *vertical, int *sdisp, int *inv)
 {
@@ -384,36 +390,36 @@ CTU_FN void ang_params(int mode, bool *vertical, int *sdisp, int *inv)
 
 // difference block (prediction - source) of the w8 x w8 sub-block at (bx, by) of mode m into d[], row-major, in the
 // mode's own orientation (transposed for horizontal modes)
-template <int W8>
-CTU_FN void rough_diff_block(const IntraRefs *r, const RoughExt *ext, int log2w, int color, int m, const uint8_t *src, int src_stride, int bx, int by, int *d)
+template <int W8, typename Pix>
+CTU_FN void rough_diff_block(const IntraRefs<Pix> *r, const RoughExt<Pix> *ext, int log2w, int color, int m, const Pix *src, int src_stride, int bx, int by, int *d)
 {
   const int w = 1 << log2w;
   if (m >= 2) {
     bool vertical; int sdisp, inv;
     ang_params(m, &vertical, &sdisp, &inv);
-    const uint8_t *e = ext->e[m - 2] + w;
+    const Pix *e = ext->e[m - 2] + w;
     // transposed domain of a horizontal mode: row index <-> picture column
     const int ox = vertical ? bx : by, oy = vertical ? by : bx;
     const int sx = vertical ? 1 : src_stride, sy = vertical ? src_stride : 1;
     const bool f = intra_uses_filtered(log2w, m, color);
-    const uint8_t *side = vertical ? (f ? r->fleft : r->left) : (f ? r->ftop : r->top);
+    const Pix *side = vertical ? (f ? r->fleft : r->left) : (f ? r->ftop : r->top);
     const bool edge = color == 0 && log2w < 5 && sdisp == 0 && ox == 0;      // modes 10 / 26: first column filtered
 #pragma unroll
     for (int y = 0; y < W8; ++y) {
       const int pos = (oy + y + 1) * sdisp;
       const int di = pos >> 5, df = pos & 31;
-      const uint8_t *p = e + ox + di;
+      const Pix *p = e + ox + di;
 #pragma unroll
       for (int x = 0; x < W8; ++x) {
         int v = ((32 - df) * (int)p[x] + df * (int)p[x + 1] + 16) >> 5;
-        if (edge && x == 0) v = iclip(0, 255, v + (((int)side[oy + y + 1] - (int)side[0]) >> 1));
+        if (edge && x == 0) v = iclip(0, PixTraits<Pix>::max, v + (((int)side[oy + y + 1] - (int)side[0]) >> 1));
         d[y * W8 + x] = v - (int)src[(oy + y) * sy + (ox + x) * sx];
       }
     }
   } else {
     // planar (filtered references for luma blocks above 4x4) and DC (unfiltered, edge-filtered for luma below 32x32)
     const bool f = intra_uses_filtered(log2w, m, color);
-    const uint8_t *t = f ? r->ftop : r->top, *l = f ? r->fleft : r->left;
+    const Pix *t = f ? r->ftop : r->top, *l = f ? r->fleft : r->left;
     const int tr = t[w + 1], bl = l[w + 1], dc = r->dc;
     const bool dc_edges = color == 0 && log2w < 5;
 #pragma unroll
@@ -440,7 +446,7 @@ CTU_FN void rough_diff_block(const IntraRefs *r, const RoughExt *ext, int log2w,
 
 // SATD (satd_NxN) and, for 4x4, SAD of the prediction of every mode against the source block.
 // satd_out / sad_out: [35] ints.  `ext`: scratch (the arena: no transform-unit job is running during the rough search).
-CTU_FN_NOINLINE void rough_costs_all_modes(const IntraRefs *r, RoughExt *ext, int log2w, int color, const uint8_t *src, int src_stride,
+template <typename Pix> CTU_FN_NOINLINE void rough_costs_all_modes(const IntraRefs<Pix> *r, RoughExt<Pix> *ext, int log2w, int color, const Pix *src, int src_stride,
                                   int32_t *satd_out, int32_t *sad_out, bool want_sad)
 {
   const int w = 1 << log2w;
@@ -454,12 +460,12 @@ CTU_FN_NOINLINE void rough_costs_all_modes(const IntraRefs *r, RoughExt *ext, in
     bool vertical; int sdisp, inv;
     ang_params(m, &vertical, &sdisp, &inv);
     const bool f = intra_uses_filtered(log2w, m, color);
-    const uint8_t *t = f ? r->ftop : r->top, *l = f ? r->fleft : r->left;
-    const uint8_t *rmain = vertical ? t : l, *rside = vertical ? l : t;
+    const Pix *t = f ? r->ftop : r->top, *l = f ? r->fleft : r->left;
+    const Pix *rmain = vertical ? t : l, *rside = vertical ? l : t;
     int v = 0;
     if (idx >= -1) { if (idx + 1 <= 2 * w) v = rmain[idx + 1]; }
     else if (sdisp < 0) v = rside[(128 + (-idx - 1) * inv) >> 8];
-    ext->e[m - 2][idx + w] = (uint8_t)v;
+    ext->e[m - 2][idx + w] = (Pix)v;
   }
   CTU_SYNC();
   if (w == 4) {
@@ -483,10 +489,18 @@ CTU_FN_NOINLINE void rough_costs_all_modes(const IntraRefs *r, RoughExt *ext, in
     }
   }
   CTU_SYNC();
+  if constexpr (PixDepth<Pix>::bd != 8) {
+    // above 8 bits the reference's SATD of 8x8 and larger blocks and its SAD are scaled to 8-bit precision
+    // (strategies-picture.h:68, picture-generic.c:381, 484, 521); the 4x4 SATD is not
+    constexpr int sh = PixDepth<Pix>::bd - 8;
+    #pragma unroll 1
+    for (int m = CTU_TID; m < 35; m += CTU_NT) { if (w > 4) satd_out[m] >>= sh; sad_out[m] >>= sh; }
+    CTU_SYNC();
+  }
 }
 
 // kvz_pixels_calc_ssd over a w x w block (result in *out after the call; out must be zeroed by the leader before)
-CTU_FN_NOINLINE void ssd_block(const uint8_t *a, int sa, const uint8_t *b, int sb, int w, int32_t *out)
+template <typename Pix> CTU_FN_NOINLINE void ssd_block(const Pix *a, int sa, const Pix *b, int sb, int w, int32_t *out)
 {
   int acc = 0;
   #pragma unroll 1
@@ -591,18 +605,18 @@ CTU_FN void quant_sign_hide_group(const SmTables *T, const int16_t *coef, int16_
 }
 
 // kvz_quant: b -> q (intra slice: rounding offset 171)
-CTU_FN_NOINLINE void quant_block(const Team &tm, const SmTables *T, const CtuConfig *cfg, const TuS &tu, int n, int type, int scan_idx)
+template <typename Pix> CTU_FN_NOINLINE void quant_block(const Team &tm, const SmTables *T, const CtuConfig *cfg, const TuS<Pix> &tu, int n, int type, int scan_idx)
 {
   const int log2n = ilog2(n);
-  const int qp_scaled = scaled_qp(type, cfg->qp);
+  const int qp_scaled = scaled_qp_px<Pix>(type, cfg->qp);
   const int qc = quant_scale(qp_scaled % 6);
-  const int transform_shift = 15 - 8 - log2n;
+  const int transform_shift = 15 - PixDepth<Pix>::bd - log2n;
   const int q_bits = 14 + qp_scaled / 6 + transform_shift;
   const int add = 171 << (q_bits - 9);
   const int q_bits8 = q_bits - 8;
   int16_t *b = tu.b(), *q = tu.q();
   int32_t *d = tu.d();
-  TuFixed *fx = tu.fx();
+  TuFixed<Pix> *fx = tu.fx();
   if (tm.tid == 0) fx->ac_sum = 0;
   tsync(tm);
   int ac = 0;
@@ -635,12 +649,12 @@ CTU_FN_NOINLINE void quant_block(const Team &tm, const SmTables *T, const CtuCon
 }
 
 // kvz_dequant: q -> b.  type: 0 luma, 2 / 3 chroma
-template <int L2N>
-CTU_FN_NOINLINE void dequant_block(const Team &tm, const CtuConfig *cfg, const TuS &tu, int n_rt, int type)
+template <int L2N, typename Pix>
+CTU_FN_NOINLINE void dequant_block(const Team &tm, const CtuConfig *cfg, const TuS<Pix> &tu, int n_rt, int type)
 {
   const int n = L2N ? (1 << L2N) : n_rt;
-  const int transform_shift = 15 - 8 - (L2N ? L2N : ilog2(n));
-  const int qp_scaled = scaled_qp(type, cfg->qp);
+  const int transform_shift = 15 - PixDepth<Pix>::bd - (L2N ? L2N : ilog2(n));
+  const int qp_scaled = scaled_qp_px<Pix>(type, cfg->qp);
   const int shift = 20 - 14 - transform_shift;
   const int scale = inv_quant_scale(qp_scaled % 6) << (qp_scaled / 6);
   const int add = 1 << (shift - 1);
@@ -700,11 +714,11 @@ CTU_FN int sig_ctx_inc(const SmTables *T, int pattern, int scan_idx, int px, int
 }
 
 // kvz_rdoq_sign_hiding (ref: rdo.c:518-653); serial, one thread
-CTU_FN_NOINLINE void rdoq_sign_hiding(const TuS &tu, const uint16_t *blk, double lambda, int qp_scaled, int last_pos, const int16_t *coef, int16_t *q)
+template <typename Pix> CTU_FN_NOINLINE void rdoq_sign_hiding(const TuS<Pix> &tu, const uint16_t *blk, double lambda, int qp_scaled, int last_pos, const int16_t *coef, int16_t *q)
 {
   const int32_t *s_inc = tu.inc(), *s_dec = tu.dec(), *s_sig_inc = tu.sig_inc(), *s_qdelta = tu.qdelta();
   const int inv_quant = inv_quant_scale(qp_scaled % 6);
-  const long long rd_factor = (long long)(inv_quant * inv_quant * (1 << (2 * (qp_scaled / 6))) / lambda / 16 / (1 << (2 * (8 - 8))) + 0.5);
+  const long long rd_factor = (long long)(inv_quant * inv_quant * (1 << (2 * (qp_scaled / 6))) / lambda / 16 / (1 << (2 * (PixDepth<Pix>::bd - 8))) + 0.5);
   const int last_cg = (last_pos - 1) >> 4;
   for (int cg = last_cg; cg >= 0; --cg) {
     const uint16_t *pos = blk + (cg << 4);
@@ -761,31 +775,31 @@ CTU_FN int team_sum(int v) { return v; }
 
 // kvz_rdoq for one TU, executed by one team (the first warp): coef = tu->b, levels to tu->q.  `cabac` = the models of
 // state->cabac (NOT the search copy: rdo.c:665).  type 0 luma / 2 chroma; tr_depth as in quant-generic.c:237-238.
-template <int L2N>
-CTU_FN_NOINLINE void rdoq_team(const SmTables *T, const SmTables *tb, const CtuConfig *cfg, const uint8_t *cabac, const TuS &tu, int log2n_rt, int type,
+template <int L2N, typename Pix>
+CTU_FN_NOINLINE void rdoq_team(const SmTables *T, const SmTables *tb, const CtuConfig *cfg, const uint8_t *cabac, const TuS<Pix> &tu, int log2n_rt, int type,
                       int scan_idx, int tr_depth, int lane)
 {
   const int log2n = L2N ? L2N : log2n_rt;
   const int16_t *coef = tu.b();
   int16_t *q = tu.q();
-  TuFixed &s = *tu.fx();
+  TuFixed<Pix> &s = *tu.fx();
   double *s_cost_coeff = tu.cost_coeff(), *s_cg_sig_cost = tu.cg_sig_cost();
   uint8_t *s_sig_code = tu.sig_code();
   int32_t *s_inc = tu.inc(), *s_dec = tu.dec(), *s_sig_inc = tu.sig_inc(), *s_qdelta = tu.qdelta(), *s_cg_flag = tu.cg_flag();
   uint16_t *s_cg_nz = tu.cg_nz();
   const int n = 1 << log2n, nn = n * n;
-  const int transform_shift = 15 - 8 - log2n;
-  const int qp_scaled = scaled_qp(type, cfg->qp);
+  const int transform_shift = 15 - PixDepth<Pix>::bd - log2n;
+  const int qp_scaled = scaled_qp_px<Pix>(type, cfg->qp);
   const int q_bits = 14 + qp_scaled / 6 + transform_shift;
   const int qc = quant_scale(qp_scaled % 6);
   const int half = 1 << (q_bits - 1);
   const double lambda = cfg->lambda;
   const bool SH = cfg->signhide_enable != 0;
-  // error scale (scalinglist.c:351-368): 2^15 * 2^(-2 * transform_shift) / q / q
+  // error scale (scalinglist.c:351-368): 2^15 * 2^(-2 * transform_shift) / q / q / 2^(2 * (bd - 8))
   double err_scale = 32768.0;
   for (int i = 0; i < 2 * transform_shift; ++i) err_scale *= 0.5;
   for (int i = 0; i > 2 * transform_shift; --i) err_scale *= 2.0;
-  err_scale = err_scale / qc / qc / 1;
+  err_scale = err_scale / qc / qc / (1 << (2 * (PixDepth<Pix>::bd - 8)));
   RdoqModels m;
   m.eb = tb->ebits;
   m.sig = cabac + (type ? CTX_SIG_CHROMA : CTX_SIG_LUMA);
@@ -1198,29 +1212,29 @@ CTU_FN_NOINLINE double coeff_cost_serial(const SmTables *T, const SmTables *tb, 
 // team's scratch: prediction, residual, transform (or transform skip), RDOQ / quantisation, and when a level
 // survived dequantisation, inverse transform and reconstruction; plus the SSD against the source that the callers'
 // cost functions need (kvz_pixels_calc_ssd).  Results: tu.pred(), tu.q(), tu.rec(), fx->has, fx->ssd.
-struct TuJob {
-  const IntraRefs *refs;
-  const uint8_t *src;       // the unit's source pixels
+template <typename Pix> struct TuJob {
+  const IntraRefs<Pix> *refs;
+  const Pix *src;       // the unit's source pixels
   int src_stride;
   int color, log2n, mode, scan_idx;
   int rdoq_tr_depth;        // context selector of RDOQ's cbf cost (quant-generic.c:237-238)
 };
 
-template <int L2N>
-CTU_FN_NOINLINE void tu_core_t(const Team &tm, const SmTables *T, const SmTables *tb, const CtuConfig *cfg, const uint8_t *cabac0, const TuS &tu,
-                               const TuJob &j, bool use_trskip)
+template <int L2N, typename Pix>
+CTU_FN_NOINLINE void tu_core_t(const Team &tm, const SmTables *T, const SmTables *tb, const CtuConfig *cfg, const uint8_t *cabac0, const TuS<Pix> &tu,
+                               const TuJob<Pix> &j, bool use_trskip)
 {
   const int log2n = L2N ? L2N : j.log2n, n = 1 << log2n, nn = n * n;
   const int color = j.color;
-  const int ts_shift = 15 - 8 - log2n;
+  const int ts_shift = 15 - PixDepth<Pix>::bd - log2n;
   int16_t *a = tu.a(), *b = tu.b(), *q = tu.q(), *t = tu.t();
-  uint8_t *pred = tu.pred(), *rec = tu.rec();
-  TuFixed *fx = tu.fx();
+  Pix *pred = tu.pred(), *rec = tu.rec();
+  TuFixed<Pix> *fx = tu.fx();
   #pragma unroll 1
   for (int e = tm.tid; e < nn; e += tm.nt) {
     const int y = e >> log2n, x = e & (n - 1);
     const int p = intra_predict_px(j.refs, log2n, j.mode, color, x, y);
-    pred[e] = (uint8_t)p;
+    pred[e] = (Pix)p;
     a[e] = (int16_t)((int)j.src[y * j.src_stride + x] - p);
   }
   if (tm.tid == 0) { fx->has = 0; fx->ssd = 0; fx->cg_mask[0] = 0; fx->cg_mask[1] = 0; }
@@ -1232,7 +1246,7 @@ CTU_FN_NOINLINE void tu_core_t(const Team &tm, const SmTables *T, const SmTables
     for (int e = tm.tid; e < nn; e += tm.nt) b[e] = (int16_t)((uint16_t)a[e] << ts_shift);
     tsync(tm);
   } else {
-    fwd_pass<L2N>(tm, a, t, M, n, log2n - 1);
+    fwd_pass<L2N>(tm, a, t, M, n, log2n - 1 + (PixDepth<Pix>::bd - 8));
     fwd_pass<L2N>(tm, t, b, M, n, log2n + 6);
   }
   const int type = color == 0 ? 0 : 2;
@@ -1267,14 +1281,14 @@ CTU_FN_NOINLINE void tu_core_t(const Team &tm, const SmTables *T, const SmTables
       tsync(tm);
     } else {
       inv_pass<L2N>(tm, b, t, M, n, 7);
-      inv_pass<L2N>(tm, t, a, M, n, 12);
+      inv_pass<L2N>(tm, t, a, M, n, 12 - (PixDepth<Pix>::bd - 8));
     }
     #pragma unroll 1
     for (int e = tm.tid; e < nn; e += tm.nt) {
       const int y = e >> log2n, x = e & (n - 1);
       const int16_t val = (int16_t)(a[e] + (int)pred[e]);
-      const int r = iclip(0, 255, (int)val);
-      rec[e] = (uint8_t)r;
+      const int r = iclip(0, PixTraits<Pix>::max, (int)val);
+      rec[e] = (Pix)r;
       const int d = (int)j.src[y * j.src_stride + x] - r;
       ssd += d * d;
     }
@@ -1283,17 +1297,22 @@ CTU_FN_NOINLINE void tu_core_t(const Team &tm, const SmTables *T, const SmTables
     for (int e = tm.tid; e < nn; e += tm.nt) {
       const int y = e >> log2n, x = e & (n - 1);
       const int r = pred[e];
-      rec[e] = (uint8_t)r;
+      rec[e] = (Pix)r;
       const int d = (int)j.src[y * j.src_stride + x] - r;
       ssd += d * d;
     }
   }
   if (ssd) CTU_ATOMIC_ADD(&fx->ssd, ssd);
   tsync(tm);
+  if constexpr (PixDepth<Pix>::bd != 8) {
+    // kvz_pixels_calc_ssd scales the unit's SSD to 8-bit precision (picture-generic.c:550)
+    if (tm.tid == 0) fx->ssd >>= 2 * (PixDepth<Pix>::bd - 8);
+    tsync(tm);
+  }
 }
 
-CTU_FN void tu_core(const Team &tm, const SmTables *T, const SmTables *tb, const CtuConfig *cfg, const uint8_t *cabac0, const TuS &tu,
-                    const TuJob &j, bool use_trskip)
+template <typename Pix> CTU_FN void tu_core(const Team &tm, const SmTables *T, const SmTables *tb, const CtuConfig *cfg, const uint8_t *cabac0, const TuS<Pix> &tu,
+                    const TuJob<Pix> &j, bool use_trskip)
 {
   if (j.log2n == 2) tu_core_t<2>(tm, T, tb, cfg, cabac0, tu, j, use_trskip);
   else tu_core_t<0>(tm, T, tb, cfg, cabac0, tu, j, use_trskip);
@@ -1302,14 +1321,14 @@ CTU_FN void tu_core(const Team &tm, const SmTables *T, const SmTables *tb, const
 // One colour of one transform unit including the transform-skip decision of 4x4 luma units
 // (kvz_quantize_residual_trskip, ref: transform.c:242-288).  `sc`: the search models the decision's bit costs read.
 // Returns tr_skip (uniform over the team); the chosen alternative is in tu.q() / tu.rec() / fx->has / fx->ssd.
-CTU_FN_NOINLINE int tu_eval(const Team &tm, const SmTables *T, const SmTables *tb, const CtuConfig *cfg, const uint8_t *cabac0, CabacState *sc,
-                            const TuS &tu, const TuJob &j)
+template <typename Pix> CTU_FN_NOINLINE int tu_eval(const Team &tm, const SmTables *T, const SmTables *tb, const CtuConfig *cfg, const uint8_t *cabac0, CabacState *sc,
+                            const TuS<Pix> &tu, const TuJob<Pix> &j)
 {
   if (!(j.log2n == 2 && j.color == 0 && cfg->trskip_enable)) {
     tu_core(tm, T, tb, cfg, cabac0, tu, j, false);
     return 0;
   }
-  TuFixed *fx = tu.fx();
+  TuFixed<Pix> *fx = tu.fx();
   for (int k = 0; k < 2; ++k) {
     tu_core(tm, T, tb, cfg, cabac0, tu, j, k == 1);
     #pragma unroll 1

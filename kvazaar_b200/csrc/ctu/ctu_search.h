@@ -11,7 +11,7 @@
 //   cu_rd_cost_tr_split_accurate,
 //   calc_mode_bits                            src/search.c:253-582
 //   kvz_mock_encode_coding_unit               src/encode_coding_tree.c:977-1075
-// Scope: tr_depth_intra = 0, pu_depth_intra.min >= 1, rdo 0..3, no lossless, 8-bit 4:2:0.
+// Scope: tr_depth_intra = 0, pu_depth_intra.min >= 1, rdo 0..3, no lossless, 8- or 10-bit 4:2:0.
 //
 // The mode decisions are the reference's: same candidate order, same double-precision cost expressions in the same
 // operation order (the build uses -fmad=false), same CABAC model adaptation.  What differs is how the work is laid
@@ -40,7 +40,7 @@ struct SearchFrame {
 
 struct TuRes { int32_t ssd, has, tr_skip, pad; double bits; uint64_t cg_mask; };
 
-struct CtuS {                       // per-CTA scalar state + scratch; shared memory on the device
+template <typename Pix> struct CtuST {                       // per-CTA scalar state + scratch; shared memory on the device
   int32_t leader_tid;               // MUST be first: CTU_LEADER_TID reads it through the raw shared-memory symbol
   int32_t pad0[3];
   CabacState cabac0;                // state->cabac: the real coder's models when the CTU starts (constant)
@@ -48,7 +48,7 @@ struct CtuS {                       // per-CTA scalar state + scratch; shared me
   CabacState tmp;                   // temp_cabac of the combined-CU path (search.c:989)
   SearchFrame fr[5];
   double ret_cost;
-  IntraRefs refs[3];
+  IntraRefs<Pix> refs[3];
   int32_t satd[35], sad[35];
   double rc0[35], rc1[35], rmb[35];   // rough cost of a mode read with state->cabac / the search models, lambda_sqrt * mode bits
   int8_t modes[40];
@@ -64,7 +64,7 @@ struct CtuS {                       // per-CTA scalar state + scratch; shared me
   int32_t best_mode;
   double best_cost;
   SmTables tb;
-  LcuLevel lv[5];                   // work tree: CU records here, planes in CtuWork::store
+  LcuLevel<Pix> lv[5];                   // work tree: CU records here, planes in CtuWork::store
   TuRes res[CTU_RDO_CANDS][3];      // [RDO candidate][colour]
   TuRes res_ts[CTU_RDO_CANDS][2];   // [RDO candidate][transform, transform skip] of a 4x4 luma unit
   // the coefficients of the transform units reconstructed last (the CU whose cost is computed next), per colour
@@ -76,13 +76,15 @@ struct CtuS {                       // per-CTA scalar state + scratch; shared me
 #endif
   alignas(16) unsigned char arena[CTU_ARENA_BYTES];
 };
+using CtuS = CtuST<uint8_t>;          // (8-bit alias, see CtuWork)
 
-struct Ctx {
+template <typename Pix> struct CtxT {
   const CtuTables *T;
   const CtuConfig *cfg;
-  CtuWork *W;
-  CtuS *S;
+  CtuWorkT<Pix> *W;
+  CtuST<Pix> *S;
 };
+using Ctx = CtxT<uint8_t>;
 
 // ------------------------------------------------------------------------------------------------ MPM, mode bits
 // kvz_intra_get_dir_luma_predictor (ref: intra.c:84-127)
@@ -101,7 +103,7 @@ CTU_FN void intra_mpm(int y, const CuRec *left, const CuRec *above, int8_t *pred
   }
 }
 // kvz_luma_mode_bits (ref: search_intra.c:641-679); leader only
-CTU_FN double luma_mode_bits(const Ctx &c, int mode, const int8_t *preds)
+template <typename Pix> CTU_FN double luma_mode_bits(const CtxT<Pix> &c, int mode, const int8_t *preds)
 {
   double bits = 0;
   const bool in = mode == preds[0] || mode == preds[1] || mode == preds[2];
@@ -111,7 +113,7 @@ CTU_FN double luma_mode_bits(const Ctx &c, int mode, const int8_t *preds)
   return bits;
 }
 // kvz_chroma_mode_bits (ref: search_intra.c:682-701); leader only
-CTU_FN double chroma_mode_bits(const Ctx &c, int chroma_mode, int luma_mode)
+template <typename Pix> CTU_FN double chroma_mode_bits(const CtxT<Pix> &c, int chroma_mode, int luma_mode)
 {
   double bits = 0;
   cabac_bin(&c.S->tb, &c.S->sc, CTX_CHROMA_PRED, chroma_mode != luma_mode, &bits);
@@ -120,7 +122,7 @@ CTU_FN double chroma_mode_bits(const Ctx &c, int chroma_mode, int luma_mode)
 }
 
 // ------------------------------------------------------------------------------------------------ work tree copies
-CTU_FN void copy_cu_info(LcuLevel *from, LcuLevel *to, int xl, int yl, int width)
+template <typename Pix> CTU_FN void copy_cu_info(LcuLevel<Pix> *from, LcuLevel<Pix> *to, int xl, int yl, int width)
 {
   const int n = width >> 2;
   #pragma unroll 1
@@ -129,7 +131,7 @@ CTU_FN void copy_cu_info(LcuLevel *from, LcuLevel *to, int xl, int yl, int width
     *cu_at(to, x, y) = *cu_at(from, x, y);
   }
 }
-CTU_FN void copy_cu_pixels(LcuLevel *from, LcuLevel *to, int xl, int yl, int width)
+template <typename Pix> CTU_FN void copy_cu_pixels(LcuLevel<Pix> *from, LcuLevel<Pix> *to, int xl, int yl, int width)
 {
   #pragma unroll 1
   for (int e = CTU_TID; e < width * width; e += CTU_NT) {
@@ -144,7 +146,7 @@ CTU_FN void copy_cu_pixels(LcuLevel *from, LcuLevel *to, int xl, int yl, int wid
     to->rec_v[y * 32 + x] = from->rec_v[y * 32 + x];
   }
 }
-CTU_FN void copy_cu_coeffs(LcuLevel *from, LcuLevel *to, int xl, int yl, int width)
+template <typename Pix> CTU_FN void copy_cu_coeffs(LcuLevel<Pix> *from, LcuLevel<Pix> *to, int xl, int yl, int width)
 {
   const int zl = zorder(64, xl, yl);
   #pragma unroll 1
@@ -153,7 +155,7 @@ CTU_FN void copy_cu_coeffs(LcuLevel *from, LcuLevel *to, int xl, int yl, int wid
   #pragma unroll 1
   for (int e = CTU_TID; e < wc * wc; e += CTU_NT) { to->coeff_u[zc + e] = from->coeff_u[zc + e]; to->coeff_v[zc + e] = from->coeff_v[zc + e]; }
 }
-CTU_FN_NOINLINE void work_tree_copy_up(const Ctx &c, int xl, int yl, int depth)
+template <typename Pix> CTU_FN_NOINLINE void work_tree_copy_up(const CtxT<Pix> &c, int xl, int yl, int depth)
 {
   const int w = 64 >> depth;
   PROF_T0(PR_COPY);
@@ -163,7 +165,7 @@ CTU_FN_NOINLINE void work_tree_copy_up(const Ctx &c, int xl, int yl, int depth)
   CTU_SYNC();
   PROF_ADD(c.S, PR_COPY);
 }
-CTU_FN_NOINLINE void work_tree_copy_down(const Ctx &c, int xl, int yl, int depth)
+template <typename Pix> CTU_FN_NOINLINE void work_tree_copy_down(const CtxT<Pix> &c, int xl, int yl, int depth)
 {
   const int w = 64 >> depth;
   PROF_T0(PR_COPY);
@@ -175,7 +177,7 @@ CTU_FN_NOINLINE void work_tree_copy_down(const Ctx &c, int xl, int yl, int depth
   PROF_ADD(c.S, PR_COPY);
 }
 // kvz_lcu_fill_trdepth
-CTU_FN_NOINLINE void fill_trdepth(LcuLevel *L, int xl, int yl, int depth, int tr_depth)
+template <typename Pix> CTU_FN_NOINLINE void fill_trdepth(LcuLevel<Pix> *L, int xl, int yl, int depth, int tr_depth)
 {
   const int n = (64 >> depth) >> 2;
   #pragma unroll 1
@@ -183,7 +185,7 @@ CTU_FN_NOINLINE void fill_trdepth(LcuLevel *L, int xl, int yl, int depth, int tr
   CTU_SYNC();
 }
 // lcu_fill_cu_info (intra fields only); `cu` may alias one of the targets
-CTU_FN_NOINLINE void fill_cu_info(LcuLevel *L, int xl, int yl, int width, const CuRec *cu)
+template <typename Pix> CTU_FN_NOINLINE void fill_cu_info(LcuLevel<Pix> *L, int xl, int yl, int width, const CuRec *cu)
 {
   const CuRec v = *cu;
   CTU_SYNC();
@@ -201,7 +203,7 @@ CTU_FN_NOINLINE void fill_cu_info(LcuLevel *L, int xl, int yl, int width, const 
 CTU_FN int tu_log2(int depth, int color) { return color == 0 ? 6 - depth : (depth < 4 ? 5 - depth : 2); }
 CTU_FN int stage_key_of(int xl, int yl, int depth) { return (xl << 16) | (yl << 8) | depth; }
 // coefficients of the unit of `color` at (xl, yl, depth) on level L: the staged copy when it is this unit's
-CTU_FN const int16_t *unit_coeffs(const Ctx &c, LcuLevel *L, int color, int xl, int yl, int depth, uint64_t *mask)
+template <typename Pix> CTU_FN const int16_t *unit_coeffs(const CtxT<Pix> &c, LcuLevel<Pix> *L, int color, int xl, int yl, int depth, uint64_t *mask)
 {
   *mask = CTU_NO_MASK;
   if (c.S->stage_key[color] == stage_key_of(xl, yl, depth)) { *mask = c.S->stage_mask[color]; return color == 0 ? c.S->stage_y : c.S->stage_c[color - 1]; }
@@ -209,7 +211,7 @@ CTU_FN const int16_t *unit_coeffs(const Ctx &c, LcuLevel *L, int color, int xl, 
   return (color == 1 ? L->coeff_u : L->coeff_v) + zorder(32, xl >> 1, yl >> 1);
 }
 
-CTU_FN double coeff_cost_of_unit(const Ctx &c, CabacState *sc, LcuLevel *L, int color, int xl, int yl, int depth, int log2n, int type, int scan)
+template <typename Pix> CTU_FN double coeff_cost_of_unit(const CtxT<Pix> &c, CabacState *sc, LcuLevel<Pix> *L, int color, int xl, int yl, int depth, int log2n, int type, int scan)
 {
   uint64_t mask;
   const int16_t *co = unit_coeffs(c, L, color, xl, yl, depth, &mask);
@@ -219,12 +221,12 @@ CTU_FN double coeff_cost_of_unit(const Ctx &c, CabacState *sc, LcuLevel *L, int 
 // Runs `ntasks` independent transform-unit jobs whose largest unit has nn coefficients: one warp per job when four
 // scratch slots fit the arena, otherwise the whole CTA job after job.  f(team, slot base, task) must synchronise
 // with tsync(team) only.
-template <class F> CTU_FN void for_tu_tasks(const Ctx &c, int ntasks, int nn, F f)
+template <typename Pix, class F> CTU_FN void for_tu_tasks(const CtxT<Pix> &c, int ntasks, int nn, F f)
 {
   CTU_SYNC();
-  if (CTU_NWARPS > 1 && CTU_NWARPS * tu_scratch_bytes(nn) <= CTU_ARENA_BYTES) {
+  if (CTU_NWARPS > 1 && CTU_NWARPS * tu_scratch_bytes<Pix>(nn) <= CTU_ARENA_BYTES) {
     const Team tm = team_warp();
-    unsigned char *slot = c.S->arena + (size_t)CTU_WARP * tu_scratch_bytes(nn);
+    unsigned char *slot = c.S->arena + (size_t)CTU_WARP * tu_scratch_bytes<Pix>(nn);
     for (int t = CTU_WARP; t < ntasks; t += CTU_NWARPS) f(tm, slot, t);
   } else {
     const Team tm = team_cta();
@@ -233,14 +235,14 @@ template <class F> CTU_FN void for_tu_tasks(const Ctx &c, int ntasks, int nn, F 
   CTU_SYNC();
 }
 
-CTU_FN TuS tu_at(unsigned char *slot, int nn) { TuS t; t.base = slot; t.nn = nn; t.ncg = nn >= 16 ? nn / 16 : 1; return t; }
+template <typename Pix> CTU_FN TuS<Pix> tu_at(unsigned char *slot, int nn) { TuS<Pix> t; t.base = slot; t.nn = nn; t.ncg = nn >= 16 ? nn / 16 : 1; return t; }
 
 // leaf part of kvz_intra_recon_cu + kvz_quantize_lcu_residual (ref: intra.c:676-696, transform.c:448-508): the
 // colours of the leaf are independent jobs (prediction only reads neighbours outside the unit).
 // refs_valid: bit per colour whose S->refs[] already hold this unit's references.
-CTU_FN_NOINLINE void intra_recon_leaf(const Ctx &c, LcuLevel *L, int x, int y, int depth, int mode_luma, int mode_chroma, CuRec *cur_cu, int leaf, int refs_valid)
+template <typename Pix> CTU_FN_NOINLINE void intra_recon_leaf(const CtxT<Pix> &c, LcuLevel<Pix> *L, int x, int y, int depth, int mode_luma, int mode_chroma, CuRec *cur_cu, int leaf, int refs_valid)
 {
-  CtuS *S = c.S;
+  CtuST<Pix> *S = c.S;
   const int xl = x & 63, yl = y & 63;
   CuRec *cur_tu = cu_at(L, xl, yl);
   const bool has_luma = mode_luma != -1;
@@ -261,20 +263,20 @@ CTU_FN_NOINLINE void intra_recon_leaf(const Ctx &c, LcuLevel *L, int x, int y, i
   for_tu_tasks(c, last - first + 1, 1 << (2 * tu_log2(depth, first)), [&](const Team &tm, unsigned char *slot, int t) {
     const int col = first + t;
     const int log2n = tu_log2(depth, col), n = 1 << log2n;
-    const TuS tu = tu_at(slot, n * n);
-    const Plane P = plane_of(c.W, L, col);
+    const TuS<Pix> tu = tu_at<Pix>(slot, n * n);
+    const Plane<Pix> P = plane_of(c.W, L, col);
     const int sh = col ? 1 : 0;
     const int off = (xl >> sh) + (yl >> sh) * P.lw;
     const int mode = col == 0 ? mode_luma : mode_chroma;
     // the scan follows the mode STORED in the CU record (quantize_tr_residual reads cur_pu->intra.mode_chroma, transform.c):
     // the chroma mode search predicts with its candidate while the record still holds the luma mode (bits 8.. of refs_valid)
     const int scan_mode = (col != 0 && (refs_valid >> 8)) ? (refs_valid >> 8) - 1 : mode;
-    TuJob j = { &S->refs[col], P.src + off, P.lw, col, log2n, mode, scan_order_intra(scan_mode, depth), rdoq_tr_depth };
+    TuJob<Pix> j = { &S->refs[col], P.src + off, P.lw, col, log2n, mode, scan_order_intra(scan_mode, depth), rdoq_tr_depth };
     const int ts = tu_eval(tm, &c.S->tb, &S->tb, c.cfg, S->cabac0.ctx, &S->sc, tu, j);
     // write back: reconstruction and coefficients of the level, staged copy for the cost functions
-    uint8_t *rec = P.rec + off;
+    Pix *rec = P.rec + off;
     int16_t *co = P.coeff + zorder(P.lw, xl >> sh, yl >> sh);
-    const uint8_t *r = tu.rec();
+    const Pix *r = tu.rec();
     const int16_t *q = tu.q();
     int16_t *stage = col == 0 ? S->stage_y : S->stage_c[col - 1];
     #pragma unroll 1
@@ -284,7 +286,7 @@ CTU_FN_NOINLINE void intra_recon_leaf(const Ctx &c, LcuLevel *L, int x, int y, i
       stage[e] = q[e];
     }
     if (tm.tid == 0) {
-      const TuFixed *fx = tu.fx();
+      const TuFixed<Pix> *fx = tu.fx();
       S->res[0][col].ssd = fx->ssd; S->res[0][col].has = fx->has; S->res[0][col].tr_skip = ts;
       S->stage_key[col] = stage_key_of(xl, yl, depth);
       S->stage_mask[col] = (uint64_t)fx->cg_mask[0] | ((uint64_t)fx->cg_mask[1] << 32);
@@ -307,7 +309,7 @@ CTU_FN_NOINLINE void intra_recon_leaf(const Ctx &c, LcuLevel *L, int x, int y, i
 
 // kvz_intra_recon_cu (ref: intra.c:623-698).  cur_cu == NULL: the CU record of the level at (x, y).  Leaves the SSDs
 // of the reconstructed colours in S->ssd[leaf][colour] (0 for the colours not touched).
-CTU_FN_NOINLINE void intra_recon_cu(const Ctx &c, LcuLevel *L, int x, int y, int depth, int mode_luma, int mode_chroma, CuRec *cur_cu, int refs_valid)
+template <typename Pix> CTU_FN_NOINLINE void intra_recon_cu(const CtxT<Pix> &c, LcuLevel<Pix> *L, int x, int y, int depth, int mode_luma, int mode_chroma, CuRec *cur_cu, int refs_valid)
 {
   const int xl = x & 63, yl = y & 63;
   if (cur_cu == NULL) cur_cu = cu_at(L, xl, yl);
@@ -350,9 +352,9 @@ CTU_FN_NOINLINE void intra_recon_cu(const Ctx &c, LcuLevel *L, int x, int y, int
 // models.  Except chroma at depth 4, which is reconstructed again: the candidate quantised it with the cbf context of
 // tr_depth 1 (pred_cu of search_intra_rdo), the CU's reconstruction uses its record's tr_depth 4 - depth 3 + NxN = 2
 // (rdo.c:919).
-CTU_FN_NOINLINE void write_back_candidate(const Ctx &c, LcuLevel *L, int x, int y, int depth, int mode, bool with_chroma)
+template <typename Pix> CTU_FN_NOINLINE void write_back_candidate(const CtxT<Pix> &c, LcuLevel<Pix> *L, int x, int y, int depth, int mode, bool with_chroma)
 {
-  CtuS *S = c.S;
+  CtuST<Pix> *S = c.S;
   const int xl = x & 63, yl = y & 63;
   const int last = with_chroma && depth < 4 ? 2 : 0;
   PROF_T0(PR_WRITEBACK);
@@ -362,11 +364,11 @@ CTU_FN_NOINLINE void write_back_candidate(const Ctx &c, LcuLevel *L, int x, int 
   for (int col = 0; col <= last; ++col) {
     const int log2n = tu_log2(depth, col), n = 1 << log2n;
     const int unit = col == 0 ? (ts_split ? 2 * cand + S->res[cand][0].tr_skip : cand) : cand;
-    const uint8_t *kr = (col == 0 ? c.W->cand.rec_y : c.W->cand.rec_c[col - 1]) + unit * n * n;
+    const Pix *kr = (col == 0 ? c.W->cand.rec_y : c.W->cand.rec_c[col - 1]) + unit * n * n;
     const int16_t *kq = (col == 0 ? c.W->cand.q_y : c.W->cand.q_c[col - 1]) + unit * n * n;
-    const Plane P = plane_of(c.W, L, col);
+    const Plane<Pix> P = plane_of(c.W, L, col);
     const int sh = col ? 1 : 0;
-    uint8_t *rec = P.rec + (xl >> sh) + (yl >> sh) * P.lw;
+    Pix *rec = P.rec + (xl >> sh) + (yl >> sh) * P.lw;
     int16_t *co = P.coeff + zorder(P.lw, xl >> sh, yl >> sh);
     int16_t *stage = col == 0 ? S->stage_y : S->stage_c[col - 1];
     #pragma unroll 1
@@ -397,7 +399,7 @@ CTU_FN_NOINLINE void write_back_candidate(const Ctx &c, LcuLevel *L, int x, int 
 // ------------------------------------------------------------------------------------------------ RD costs
 // kvz_cu_rd_cost_luma for a leaf (tr_depth == depth), the search models not adapting (update == 0: the candidates of
 // search_intra_rdo).  Leader only.  ssd / coeff_bits: the unit's SSD and kvz_get_coeff_cost (0 when cbf is clear).
-CTU_FN_NOINLINE double cu_rd_cost_luma_leaf(const Ctx &c, LcuLevel *L, int xl, int yl, int depth, const CuRec *pred_cu, int ssd, double coeff_bits_y)
+template <typename Pix> CTU_FN_NOINLINE double cu_rd_cost_luma_leaf(const CtxT<Pix> &c, LcuLevel<Pix> *L, int xl, int yl, int depth, const CuRec *pred_cu, int ssd, double coeff_bits_y)
 {
   CabacState *sc = &c.S->sc;
   const int width = 64 >> depth;
@@ -422,7 +424,7 @@ CTU_FN_NOINLINE double cu_rd_cost_luma_leaf(const Ctx &c, LcuLevel *L, int xl, i
 }
 
 // kvz_cu_rd_cost_chroma for a leaf, update == 0.  Leader only.
-CTU_FN_NOINLINE double cu_rd_cost_chroma_leaf(const Ctx &c, LcuLevel *L, int xl, int yl, int depth, const CuRec *pred_cu, int ssd, double coeff_bits_u, double coeff_bits_v)
+template <typename Pix> CTU_FN_NOINLINE double cu_rd_cost_chroma_leaf(const CtxT<Pix> &c, LcuLevel<Pix> *L, int xl, int yl, int depth, const CuRec *pred_cu, int ssd, double coeff_bits_u, double coeff_bits_v)
 {
   CabacState *sc = &c.S->sc;
   CuRec *tr_cu = cu_at(L, xl, yl);
@@ -442,7 +444,7 @@ CTU_FN_NOINLINE double cu_rd_cost_chroma_leaf(const Ctx &c, LcuLevel *L, int xl,
 }
 
 // the same with the coefficient bits taken from the level's (or staged) coefficients; S->ssd[leaf] holds the SSDs
-CTU_FN_NOINLINE double cu_rd_cost_chroma_leaf_of_level(const Ctx &c, LcuLevel *L, int xl, int yl, int depth, const CuRec *pred_cu, int leaf)
+template <typename Pix> CTU_FN_NOINLINE double cu_rd_cost_chroma_leaf_of_level(const CtxT<Pix> &c, LcuLevel<Pix> *L, int xl, int yl, int depth, const CuRec *pred_cu, int leaf)
 {
   if (xl % 8 != 0 || yl % 8 != 0) return 0;
   const CuRec *tr_cu = cu_at(L, xl, yl);
@@ -455,9 +457,9 @@ CTU_FN_NOINLINE double cu_rd_cost_chroma_leaf_of_level(const Ctx &c, LcuLevel *L
 }
 
 // cu_rd_cost_tr_split_accurate (ref: search.c:414-543), one node.  Leader only.  `leaf`: index into S->ssd.
-CTU_FN_NOINLINE double cost_accurate_node(const Ctx &c, LcuLevel *L, int xl, int yl, int depth, const CuRec *pred_cu, int leaf, bool *is_split)
+template <typename Pix> CTU_FN_NOINLINE double cost_accurate_node(const CtxT<Pix> &c, LcuLevel<Pix> *L, int xl, int yl, int depth, const CuRec *pred_cu, int leaf, bool *is_split)
 {
-  const CtuS *S = c.S;
+  const CtuST<Pix> *S = c.S;
   CabacState *sc = &c.S->sc;
   const int width = 64 >> depth;
   CuRec *tr_cu = cu_at(L, xl, yl);
@@ -494,7 +496,7 @@ CTU_FN_NOINLINE double cost_accurate_node(const Ctx &c, LcuLevel *L, int xl, int
   const double bits = tr_tree_bits + coeff_bits;
   return luma_ssd * 0.8 + chroma_ssd * 1.5 + bits * c.cfg->lambda;
 }
-CTU_FN_NOINLINE double cost_tr_split_accurate(const Ctx &c, LcuLevel *L, int xl, int yl, int depth, const CuRec *pred_cu)
+template <typename Pix> CTU_FN_NOINLINE double cost_tr_split_accurate(const CtxT<Pix> &c, LcuLevel<Pix> *L, int xl, int yl, int depth, const CuRec *pred_cu)
 {
   bool split = false;
   const double v = cost_accurate_node(c, L, xl, yl, depth, pred_cu, 0, &split);
@@ -509,7 +511,7 @@ CTU_FN_NOINLINE double cost_tr_split_accurate(const Ctx &c, LcuLevel *L, int xl,
 }
 
 // calc_mode_bits (ref: search.c:557-582).  Leader only.
-CTU_FN double calc_mode_bits(const Ctx &c, LcuLevel *L, const CuRec *cur_cu, int x, int y)
+template <typename Pix> CTU_FN double calc_mode_bits(const CtxT<Pix> &c, LcuLevel<Pix> *L, const CuRec *cur_cu, int x, int y)
 {
   const int xl = x & 63, yl = y & 63;
   int8_t cand[3];
@@ -523,7 +525,7 @@ CTU_FN double calc_mode_bits(const Ctx &c, LcuLevel *L, const CuRec *cur_cu, int
 
 // kvz_mock_encode_coding_unit for an intra CU in an I slice (ref: encode_coding_tree.c:977-1075, 464-652, 672-743).
 // Leader only.
-CTU_FN_NOINLINE double mock_encode_coding_unit(const Ctx &c, LcuLevel *L, int x, int y, int depth, const CuRec *cur_cu)
+template <typename Pix> CTU_FN_NOINLINE double mock_encode_coding_unit(const CtxT<Pix> &c, LcuLevel<Pix> *L, int x, int y, int depth, const CuRec *cur_cu)
 {
   double bits = 0;
   CabacState *sc = &c.S->sc;
@@ -591,9 +593,9 @@ CTU_FN void sort_modes(int8_t *modes, double *costs, int length)
 
 // The per-mode quantities of search_intra_rough (get_cost / get_cost_dual, search_intra.c:89-160, and the mode bits
 // added at :524) for all 35 modes, one mode per thread.
-CTU_FN_NOINLINE void rough_mode_costs(const Ctx &c, int log2w, const int8_t *mpm)
+template <typename Pix> CTU_FN_NOINLINE void rough_mode_costs(const CtxT<Pix> &c, int log2w, const int8_t *mpm)
 {
-  CtuS *S = c.S;
+  CtuST<Pix> *S = c.S;
   const CtuConfig *cfg = c.cfg;
   const bool ts = log2w == 2 && cfg->trskip_enable;
   #pragma unroll 1
@@ -622,9 +624,9 @@ CTU_FN_NOINLINE void rough_mode_costs(const Ctx &c, int log2w, const int8_t *mpm
 }
 
 // search_intra_rough (ref: search_intra.c:391-530) replayed on the per-mode tables.  Leader only.
-CTU_FN_NOINLINE int rough_search_replay(const Ctx &c, int log2w, const int8_t *mpm)
+template <typename Pix> CTU_FN_NOINLINE int rough_search_replay(const CtxT<Pix> &c, int log2w, const int8_t *mpm)
 {
-  CtuS *S = c.S;
+  CtuST<Pix> *S = c.S;
   const CtuConfig *cfg = c.cfg;
   int8_t *modes = S->modes;
   double *costs = S->costs;
@@ -673,9 +675,9 @@ CTU_FN_NOINLINE int rough_search_replay(const Ctx &c, int log2w, const int8_t *m
 }
 
 // copy of a transform-unit job's reconstruction and levels (team)
-CTU_FN_NOINLINE void keep_unit(const Team &tm, const TuS &tu, uint8_t *kr, int16_t *kq)
+template <typename Pix> CTU_FN_NOINLINE void keep_unit(const Team &tm, const TuS<Pix> &tu, Pix *kr, int16_t *kq)
 {
-  const uint8_t *r = tu.rec();
+  const Pix *r = tu.rec();
   const int16_t *q = tu.q();
   #pragma unroll 1
   for (int e = tm.tid; e < tu.nn; e += tm.nt) { kr[e] = r[e]; kq[e] = q[e]; }
@@ -683,9 +685,9 @@ CTU_FN_NOINLINE void keep_unit(const Team &tm, const TuS &tu, uint8_t *kr, int16
 
 // kvz_search_cu_intra (ref: search_intra.c:806-900): best luma mode of the CU at (x, y, depth) on level L.
 // Result in S->best_mode / S->best_cost.
-CTU_FN_NOINLINE void search_cu_intra(const Ctx &c, LcuLevel *L, int x, int y, int depth)
+template <typename Pix> CTU_FN_NOINLINE void search_cu_intra(const CtxT<Pix> &c, LcuLevel<Pix> *L, int x, int y, int depth)
 {
-  CtuS *S = c.S;
+  CtuST<Pix> *S = c.S;
   const CtuConfig *cfg = c.cfg;
   const int xl = x & 63, yl = y & 63;
   const int log2w = 6 - depth;
@@ -704,7 +706,7 @@ CTU_FN_NOINLINE void search_cu_intra(const Ctx &c, LcuLevel *L, int x, int y, in
   PROF_ADD(S, PR_REFS);
   // rough search: SATD (and SAD for 4x4 transform-skip candidates) of every mode, then the reference's selection
   PROF_T0(PR_SATD);
-  rough_costs_all_modes(&S->refs[0], (RoughExt *)S->arena, log2w, 0, &c.W->src_y[yl * 64 + xl], 64, S->satd, S->sad, log2w == 2 && cfg->trskip_enable);
+  rough_costs_all_modes(&S->refs[0], (RoughExt<Pix> *)S->arena, log2w, 0, &c.W->src_y[yl * 64 + xl], 64, S->satd, S->sad, log2w == 2 && cfg->trskip_enable);
   PROF_ADD(S, PR_SATD);
   PROF_T0(PR_REPLAY);
   rough_mode_costs(c, log2w, S->mpm);
@@ -747,23 +749,23 @@ CTU_FN_NOINLINE void search_cu_intra(const Ctx &c, LcuLevel *L, int x, int y, in
       const int col = k < nluma ? 0 : 1 + (k - nluma);
       const int mode = S->modes[cand];
       const int log2n = tu_log2(depth, col), n = 1 << log2n;
-      const TuS tu = tu_at(slot, n * n);
-      const Plane P = plane_of(c.W, L, col);
+      const TuS<Pix> tu = tu_at<Pix>(slot, n * n);
+      const Plane<Pix> P = plane_of(c.W, L, col);
       const int sh = col ? 1 : 0;
       const int off = (xl >> sh) + (yl >> sh) * P.lw;
-      TuJob j = { &S->refs[col], P.src + off, P.lw, col, log2n, mode, scan_order_intra(mode, depth), rdoq_tr_depth };
+      TuJob<Pix> j = { &S->refs[col], P.src + off, P.lw, col, log2n, mode, scan_order_intra(mode, depth), rdoq_tr_depth };
       int ts = 0;
       if (col == 0 && ts_split) tu_core(tm, &c.S->tb, &S->tb, cfg, S->cabac0.ctx, tu, j, k == 1);
       else ts = tu_eval(tm, &c.S->tb, &S->tb, cfg, S->cabac0.ctx, &S->sc, tu, j);
       // keep the unit for write_back_candidate (not the chroma of depth 4, which is quantised again: see there)
       if (col == 0 || depth < 4) {
         const int unit = col == 0 ? cand * nluma + k : cand;
-        uint8_t *kr = (col == 0 ? c.W->cand.rec_y : c.W->cand.rec_c[col - 1]) + unit * n * n;
+        Pix *kr = (col == 0 ? c.W->cand.rec_y : c.W->cand.rec_c[col - 1]) + unit * n * n;
         int16_t *kq = (col == 0 ? c.W->cand.q_y : c.W->cand.q_c[col - 1]) + unit * n * n;
         keep_unit(tm, tu, kr, kq);
       }
       if (tm.tid == 0) {
-        const TuFixed *fx = tu.fx();
+        const TuFixed<Pix> *fx = tu.fx();
         TuRes *r = (col == 0 && ts_split) ? &S->res_ts[cand][k] : &S->res[cand][col];
         r->ssd = fx->ssd; r->has = fx->has; r->tr_skip = ts;
         r->cg_mask = (uint64_t)fx->cg_mask[0] | ((uint64_t)fx->cg_mask[1] << 32);
@@ -824,9 +826,9 @@ CTU_FN_NOINLINE void search_cu_intra(const Ctx &c, LcuLevel *L, int x, int y, in
 }
 
 // kvz_search_cu_intra_chroma (ref: search_intra.c:748-803) for rdo 2..3 (num_modes = 2).  Returns the mode (uniform).
-CTU_FN_NOINLINE int search_cu_intra_chroma(const Ctx &c, LcuLevel *L, int x, int y, int depth)
+template <typename Pix> CTU_FN_NOINLINE int search_cu_intra_chroma(const CtxT<Pix> &c, LcuLevel<Pix> *L, int x, int y, int depth)
 {
-  CtuS *S = c.S;
+  CtuST<Pix> *S = c.S;
   const int xl = x & 63, yl = y & 63;
   const int intra_mode = cu_at(L, xl, yl)->mode;
   const int log2wc = imax(6 - depth - 1, 2);
@@ -841,10 +843,10 @@ CTU_FN_NOINLINE int search_cu_intra_chroma(const Ctx &c, LcuLevel *L, int x, int
   build_refs(&c.S->tb, c.cfg, c.W, L, log2wc, 2, x, y, &S->refs[2]);
   // search_intra_chroma_rough: SATD of the five candidates on U and V (the luma mode is skipped: cost 0)
   const int ci = (yl >> 1) * 32 + (xl >> 1);
-  rough_costs_all_modes(&S->refs[1], (RoughExt *)S->arena, log2wc, 1, &c.W->src_u[ci], 32, S->satd, S->sad, false);
+  rough_costs_all_modes(&S->refs[1], (RoughExt<Pix> *)S->arena, log2wc, 1, &c.W->src_u[ci], 32, S->satd, S->sad, false);
   CTU_LEADER { for (int i = 0; i < 5; ++i) S->ccosts[i] = 0; for (int i = 0; i < 5; ++i) if (S->cmodes[i] != intra_mode) S->ccosts[i] += (double)(unsigned)S->satd[S->cmodes[i]]; }
   CTU_SYNC();
-  rough_costs_all_modes(&S->refs[2], (RoughExt *)S->arena, log2wc, 2, &c.W->src_v[ci], 32, S->satd, S->sad, false);
+  rough_costs_all_modes(&S->refs[2], (RoughExt<Pix> *)S->arena, log2wc, 2, &c.W->src_v[ci], 32, S->satd, S->sad, false);
   CTU_LEADER {
     for (int i = 0; i < 5; ++i) if (S->cmodes[i] != intra_mode) S->ccosts[i] += (double)(unsigned)S->satd[S->cmodes[i]];
     sort_modes(S->cmodes, S->ccosts, 5);
@@ -885,7 +887,7 @@ CTU_FN_NOINLINE int search_cu_intra_chroma(const Ctx &c, LcuLevel *L, int x, int
 }
 
 // ------------------------------------------------------------------------------------------------ search_cu
-CTU_FN int split_model_of(LcuLevel *L, int x, int y, int depth)     // get_ctx_cu_split_model (search.c:634-641)
+template <typename Pix> CTU_FN int split_model_of(LcuLevel<Pix> *L, int x, int y, int depth)     // get_ctx_cu_split_model (search.c:634-641)
 {
   const int xl = x & 63, yl = y & 63;
   const bool condA = x >= 8 && cu_at(L, xl - 1, yl)->depth > depth;
@@ -894,9 +896,9 @@ CTU_FN int split_model_of(LcuLevel *L, int x, int y, int depth)     // get_ctx_c
 }
 
 // search_cu for the whole CTU at (cx, cy) (luma picture coordinates); returns with the decisions on level 0
-CTU_FN_NOINLINE void search_ctu(const Ctx &c, int cx, int cy)
+template <typename Pix> CTU_FN_NOINLINE void search_ctu(const CtxT<Pix> &c, int cx, int cy)
 {
-  CtuS *S = c.S;
+  CtuST<Pix> *S = c.S;
   const CtuConfig *cfg = c.cfg;
   sm_tables_load(&S->tb, c.T);
   CTU_LEADER { S->fr[0].x = cx; S->fr[0].y = cy; S->fr[0].stage = 0; S->stage_key[0] = S->stage_key[1] = S->stage_key[2] = -1; }
@@ -904,7 +906,7 @@ CTU_FN_NOINLINE void search_ctu(const Ctx &c, int cx, int cy)
   int d = 0;
   for (;;) {
     SearchFrame *F = &S->fr[d];
-    LcuLevel *L = &c.S->lv[d];
+    LcuLevel<Pix> *L = &c.S->lv[d];
     // Every thread takes its copy of the frame's state, THEN the barrier: the leader changes that state below, and a
     // thread that read it late would take another branch than the others (all control flow here must be uniform).
     const int x = F->x, y = F->y;

@@ -12,6 +12,9 @@
 //
 // Memory per picture slot: source / reconstruction / final planes, the per-4x4 CU records, 12 KB of coefficients per
 // CTU, and one work tree (CtuWork, 5 levels) per persistent CTA.
+//
+// The kernels are instantiated for 8-bit (uint8_t) and 10-bit (uint16_t) samples; kvz_cuda_ctu_open picks the pair
+// that matches kvz_cuda_ctu_config.bitdepth, and every buffer of a slot is sized in samples of that type.
 #include <time.h>
 #include <condition_variable>
 #include <mutex>
@@ -32,13 +35,17 @@ namespace {
 
 constexpr int kThreads = 128;
 // three CTAs per SM: registers (168 x 128 threads) and shared memory (228 KB per SM, 1 KB reserved per CTA)
-static_assert(sizeof(CtuS) + 1024 + 64 <= 228 * 1024 / 3, "CtuS no longer fits three CTAs per SM");
+static_assert(sizeof(CtuST<uint8_t>) + 1024 + 64 <= 228 * 1024 / 3, "CtuST<uint8_t> no longer fits three CTAs per SM");
+static_assert(sizeof(CtuST<uint16_t>) + 1024 + 64 <= 228 * 1024 / 3, "CtuST<uint16_t> no longer fits three CTAs per SM");
+#if !defined(KVZ_CTU_PROF)
+static_assert(sizeof(CtuST<uint8_t>) == 74960, "the 8-bit shared-memory layout changed");
+#endif
 
-struct KernelArgs {
+template <typename Pix> struct KernelArgs {
   const CtuTables *T;
   CtuConfig cfg;
-  FrameDev F;
-  CtuWork *work;           // [grid]
+  FrameDevT<Pix> F;
+  CtuWorkT<Pix> *work;      // [grid]
   SaoStats *sao_stats;     // [grid]
   uint8_t *dbg_ctx;        // [nctu][184] or NULL
   const uint16_t *order;   // [nctu][2]: CTU coordinates by ticket (wavefront order)
@@ -69,13 +76,14 @@ __device__ __forceinline__ void st_release(int *p, int v) { asm volatile("st.rel
 
 __device__ __forceinline__ unsigned sm_id() { unsigned v; asm volatile("mov.u32 %0, %%smid;" : "=r"(v)); return v; }
 
-__global__ void __launch_bounds__(kThreads, 3) ctu_frame_kernel(const __grid_constant__ KernelArgs a)
+template <typename Pix>
+__global__ void __launch_bounds__(kThreads, 3) ctu_frame_kernel(const __grid_constant__ KernelArgs<Pix> a)
 {
-  CtuS *S = reinterpret_cast<CtuS *>(ctu_smem_raw);
+  CtuST<Pix> *S = reinterpret_cast<CtuST<Pix> *>(ctu_smem_raw);
   __shared__ int s_ticket;
   if (threadIdx.x == 0) S->leader_tid = a.sm_counter ? 32 * (atomicAdd(a.sm_counter + (sm_id() & 255), 1) & 3) : 0;
   __syncthreads();
-  Ctx c = { a.T, &a.cfg, a.work + blockIdx.x, S };
+  CtxT<Pix> c = { a.T, &a.cfg, a.work + blockIdx.x, S };
 #if defined(KVZ_CTU_PROF)
   const long long cta_t0 = clock64();
   if (threadIdx.x == 0) for (int i = 0; i < PR_N; ++i) S->prof[i] = 0;
@@ -126,14 +134,15 @@ __global__ void __launch_bounds__(kThreads, 3) ctu_frame_kernel(const __grid_con
 }
 
 // Diagnostic alternative (KVZ_CUDA_CTU_DIAG=1): one launch per anti-diagonal, no inter-CTA waiting.
-__global__ void __launch_bounds__(kThreads, 3) ctu_diag_kernel(const __grid_constant__ KernelArgs a, int diag, int cy_lo)
+template <typename Pix>
+__global__ void __launch_bounds__(kThreads, 3) ctu_diag_kernel(const __grid_constant__ KernelArgs<Pix> a, int diag, int cy_lo)
 {
-  CtuS *S = reinterpret_cast<CtuS *>(ctu_smem_raw);
+  CtuST<Pix> *S = reinterpret_cast<CtuST<Pix> *>(ctu_smem_raw);
   if (threadIdx.x == 0) S->leader_tid = 0;
   __syncthreads();
   const int cy = cy_lo + blockIdx.x;
   const int cx = diag - 2 * cy;
-  Ctx c = { a.T, &a.cfg, a.work + blockIdx.x, S };
+  CtxT<Pix> c = { a.T, &a.cfg, a.work + blockIdx.x, S };
 #if defined(KVZ_CTU_PROF)
   if (threadIdx.x == 0) for (int i = 0; i < PR_N; ++i) S->prof[i] = 0;
   __syncthreads();
@@ -141,7 +150,8 @@ __global__ void __launch_bounds__(kThreads, 3) ctu_diag_kernel(const __grid_cons
   ctu_job(c, &a.F, reinterpret_cast<SaoStats *>(S->arena), cx, cy);
 }
 
-__global__ void __launch_bounds__(kThreads) ctu_sao_apply_kernel(const __grid_constant__ KernelArgs a)
+template <typename Pix>
+__global__ void __launch_bounds__(kThreads) ctu_sao_apply_kernel(const __grid_constant__ KernelArgs<Pix> a)
 {
   const int cy = blockIdx.x / a.F.wlcu, cx = blockIdx.x % a.F.wlcu;
   ctu_sao_apply(&a.cfg, &a.F, cx, cy);
@@ -156,26 +166,30 @@ struct Slot {
   unsigned long long seq = 0;
   bool resident = false;
   // device
-  uint8_t *d_planes = nullptr;   // src | rec | out | dbg, each w*h*3/2
+  uint8_t *d_planes = nullptr;   // src | rec | out | dbg, each w*h*3/2 samples
   uint8_t *d_bufs = nullptr;     // hor / ver buffers
   CuRec *d_cu = nullptr;
   int16_t *d_coeff = nullptr;
   SaoRec *d_sao = nullptr;
   CabacState *d_row_ctx = nullptr;
-  CtuWork *d_work = nullptr;
+  void *d_work = nullptr;        // CtuWorkT<Pix>[grid]
   SaoStats *d_stats = nullptr;
   int *d_sync = nullptr;
   uint8_t *d_dbg_ctx = nullptr;
   // pinned host
-  uint8_t *h_src = nullptr;      // staging for the upload
+  uint8_t *h_src = nullptr;      // staging for the upload (bytes, samples of the configured type)
   uint8_t *h_out = nullptr, *h_dbg = nullptr;
   CuRec *h_cu = nullptr;
   int16_t *h_coeff = nullptr;
   SaoRec *h_sao = nullptr;
   CabacState *h_row_ctx = nullptr;
   uint8_t *h_dbg_ctx = nullptr;
-  KernelArgs args;
+  KernelArgs<uint8_t> args8;     // the arguments of the instantiation in use
+  KernelArgs<uint16_t> args16;
 };
+template <typename Pix> KernelArgs<Pix> &args_of(Slot &s);
+template <> KernelArgs<uint8_t> &args_of<uint8_t>(Slot &s) { return s.args8; }
+template <> KernelArgs<uint16_t> &args_of<uint16_t>(Slot &s) { return s.args16; }
 
 }  // namespace
 
@@ -186,6 +200,7 @@ struct kvz_cuda_ctu_enc {
   unsigned long long *d_prof = nullptr;
   int *d_sm_counter = nullptr;
   int wl = 0, hl = 0, max_diag = 0, grid = 0;
+  int pix = 1;                   // bytes per sample: 1 (8-bit) or 2 (10-bit)
   size_t plane_bytes = 0, smem = 0;
   bool debug = false, diag_launches = false;
   std::vector<Slot> slots;
@@ -213,6 +228,7 @@ int kvz_cuda_ctu_config_supported(const kvz_cuda_ctu_config *c)
   if (c->rdo < 0 || c->rdo > 3) return -1;
   if (c->pu_depth_intra_min < 1 || c->pu_depth_intra_max > 4 || c->pu_depth_intra_min > c->pu_depth_intra_max) return -1;
   if (c->qp < 0 || c->qp > 51) return -1;
+  if (c->bitdepth != 0 && c->bitdepth != 8 && c->bitdepth != 10) return -1;
   return 0;
 }
 
@@ -246,6 +262,31 @@ void kvz_cuda_ctu_close(kvz_cuda_ctu_enc *e)
   delete e;
 }
 
+}  // extern "C"
+
+// kernel arguments of a slot whose buffers are allocated: planes and border buffers in samples of Pix
+template <typename Pix> static void init_args(kvz_cuda_ctu_enc *e, Slot &s, KernelArgs<Pix> &a)
+{
+  const int W = e->cfg.width, H = e->cfg.height;
+  a.T = e->d_tables;
+  a.work = (CtuWorkT<Pix> *)s.d_work; a.sao_stats = s.d_stats; a.dbg_ctx = s.d_dbg_ctx;
+  a.order = e->d_order; a.sync = s.d_sync; a.nctu = e->wl * e->hl; a.prof = e->d_prof; a.sm_counter = getenv("KVZ_CUDA_CTU_LEADER0") ? nullptr : e->d_sm_counter;   // (A/B switch: leader always warp 0)
+  FrameDevT<Pix> &F = a.F;
+  const size_t ysz = (size_t)W * H, csz = ysz / 4, plane = ysz + 2 * csz;
+  Pix *p = (Pix *)s.d_planes;
+  F.src_y = p; F.src_u = p + ysz; F.src_v = p + ysz + csz; p += plane;
+  F.rec_y = p; F.rec_u = p + ysz; F.rec_v = p + ysz + csz; p += plane;
+  F.out_y = p; F.out_u = p + ysz; F.out_v = p + ysz + csz; p += plane;
+  if (e->debug) { F.dbg_y = p; F.dbg_u = p + ysz; F.dbg_v = p + ysz + csz; } else { F.dbg_y = F.dbg_u = F.dbg_v = nullptr; }
+  Pix *b = (Pix *)s.d_bufs;
+  F.hor_y = b; b += (size_t)W * e->hl; F.hor_u = b; b += (size_t)(W / 2) * e->hl; F.hor_v = b; b += (size_t)(W / 2) * e->hl;
+  F.ver_y = b; b += (size_t)H * e->wl; F.ver_u = b; b += (size_t)(H / 2) * e->wl; F.ver_v = b;
+  F.cu = s.d_cu; F.coeff = s.d_coeff; F.sao = s.d_sao; F.row_ctx = s.d_row_ctx;
+  F.cu_stride = e->wl * 16; F.wlcu = e->wl; F.hlcu = e->hl;
+}
+
+extern "C" {
+
 kvz_cuda_ctu_enc *kvz_cuda_ctu_open(const kvz_cuda_ctu_config *cfg, int slots)
 {
   if (kvz_cuda_ctu_config_supported(cfg)) { kvzc::set_error("kvz_cuda_ctu_open: configuration outside the driver's scope"); return nullptr; }
@@ -269,8 +310,9 @@ kvz_cuda_ctu_enc *kvz_cuda_ctu_open(const kvz_cuda_ctu_config *cfg, int slots)
   e->grid = e->diag_launches ? e->max_diag : (e->max_diag * 2 + 4) / 5;
   if (e->grid < 1) e->grid = 1;
   if (const char *g = getenv("KVZ_CUDA_CTU_GRID")) { const int v = atoi(g); if (v > 0 && !e->diag_launches) e->grid = v < e->max_diag ? v : e->max_diag; }
-  e->plane_bytes = (size_t)W * H * 3 / 2;
-  e->smem = sizeof(CtuS);
+  e->pix = cfg->bitdepth == 10 ? 2 : 1;
+  e->plane_bytes = (size_t)W * H * 3 / 2 * e->pix;
+  e->smem = e->pix == 2 ? sizeof(CtuST<uint16_t>) : sizeof(CtuST<uint8_t>);
   e->debug = getenv("KVZ_CUDA_CTU_DEBUG") != nullptr;
   {
     CtuTables *ht = new CtuTables;
@@ -288,12 +330,17 @@ kvz_cuda_ctu_enc *kvz_cuda_ctu_open(const kvz_cuda_ctu_config *cfg, int slots)
   CTU_CHECK_PTR(cudaMemset(e->d_sm_counter, 0, 256 * sizeof(int)));
   CTU_CHECK_PTR(cudaMalloc(&e->d_order, order.size() * sizeof(uint16_t)));
   CTU_CHECK_PTR(cudaMemcpy(e->d_order, order.data(), order.size() * sizeof(uint16_t), cudaMemcpyHostToDevice));
-  CTU_CHECK_PTR(cudaFuncSetAttribute(ctu_frame_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)e->smem));
-  CTU_CHECK_PTR(cudaFuncSetAttribute(ctu_diag_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)e->smem));
+  if (e->pix == 2) {
+    CTU_CHECK_PTR(cudaFuncSetAttribute(ctu_frame_kernel<uint16_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)e->smem));
+    CTU_CHECK_PTR(cudaFuncSetAttribute(ctu_diag_kernel<uint16_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)e->smem));
+  } else {
+    CTU_CHECK_PTR(cudaFuncSetAttribute(ctu_frame_kernel<uint8_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)e->smem));
+    CTU_CHECK_PTR(cudaFuncSetAttribute(ctu_diag_kernel<uint8_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)e->smem));
+  }
   e->slots.resize(slots > 0 ? (slots > 512 ? 512 : slots) : 1);
   const size_t nctu = (size_t)e->wl * e->hl;
   const size_t cu_n = (size_t)(e->wl * 16) * (e->hl * 16);
-  const size_t buf_bytes = ((size_t)W * e->hl + (size_t)H * e->wl) * 2 + 64;      // Y + U + V rows (columns): w + w/2 + w/2
+  const size_t buf_bytes = (((size_t)W * e->hl + (size_t)H * e->wl) * 2 + 64) * e->pix;    // Y + U + V rows (columns): w + w/2 + w/2
   for (Slot &s : e->slots) {
     CTU_CHECK_PTR(cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking));
     CTU_CHECK_PTR(cudaEventCreateWithFlags(&s.done, cudaEventDisableTiming));
@@ -306,7 +353,7 @@ kvz_cuda_ctu_enc *kvz_cuda_ctu_open(const kvz_cuda_ctu_config *cfg, int slots)
     CTU_CHECK_PTR(cudaMalloc(&s.d_coeff, nctu * 6144 * sizeof(int16_t)));
     CTU_CHECK_PTR(cudaMalloc(&s.d_sao, nctu * 2 * sizeof(SaoRec)));
     CTU_CHECK_PTR(cudaMalloc(&s.d_row_ctx, e->hl * sizeof(CabacState)));
-    CTU_CHECK_PTR(cudaMalloc(&s.d_work, (size_t)e->grid * sizeof(CtuWork)));
+    CTU_CHECK_PTR(cudaMalloc(&s.d_work, (size_t)e->grid * (e->pix == 2 ? sizeof(CtuWorkT<uint16_t>) : sizeof(CtuWorkT<uint8_t>))));
     CTU_CHECK_PTR(cudaMalloc(&s.d_stats, (size_t)e->grid * sizeof(SaoStats)));
     CTU_CHECK_PTR(cudaMalloc(&s.d_sync, (size_t)(e->hl + 2) * sizeof(int)));
     CTU_CHECK_PTR(cudaMemset(s.d_sao, 0, nctu * 2 * sizeof(SaoRec)));
@@ -323,28 +370,43 @@ kvz_cuda_ctu_enc *kvz_cuda_ctu_open(const kvz_cuda_ctu_config *cfg, int slots)
       CTU_CHECK_PTR(cudaHostAlloc(&s.h_dbg_ctx, nctu * CTX_COUNT, cudaHostAllocDefault));
       CTU_CHECK_PTR(cudaHostAlloc(&s.h_dbg, e->plane_bytes, cudaHostAllocDefault));
     }
-    KernelArgs &a = s.args;
-    a.T = e->d_tables;
-    a.work = s.d_work; a.sao_stats = s.d_stats; a.dbg_ctx = s.d_dbg_ctx;
-    a.order = e->d_order; a.sync = s.d_sync; a.nctu = e->wl * e->hl; a.prof = e->d_prof; a.sm_counter = getenv("KVZ_CUDA_CTU_LEADER0") ? nullptr : e->d_sm_counter;   // (A/B switch: leader always warp 0)
-    FrameDev &F = a.F;
-    const size_t ysz = (size_t)W * H, csz = ysz / 4;
-    uint8_t *p = s.d_planes;
-    F.src_y = p; F.src_u = p + ysz; F.src_v = p + ysz + csz; p += e->plane_bytes;
-    F.rec_y = p; F.rec_u = p + ysz; F.rec_v = p + ysz + csz; p += e->plane_bytes;
-    F.out_y = p; F.out_u = p + ysz; F.out_v = p + ysz + csz; p += e->plane_bytes;
-    if (e->debug) { F.dbg_y = p; F.dbg_u = p + ysz; F.dbg_v = p + ysz + csz; } else { F.dbg_y = F.dbg_u = F.dbg_v = nullptr; }
-    uint8_t *b = s.d_bufs;
-    F.hor_y = b; b += (size_t)W * e->hl; F.hor_u = b; b += (size_t)(W / 2) * e->hl; F.hor_v = b; b += (size_t)(W / 2) * e->hl;
-    F.ver_y = b; b += (size_t)H * e->wl; F.ver_u = b; b += (size_t)(H / 2) * e->wl; F.ver_v = b;
-    F.cu = s.d_cu; F.coeff = s.d_coeff; F.sao = s.d_sao; F.row_ctx = s.d_row_ctx;
-    F.cu_stride = e->wl * 16; F.wlcu = e->wl; F.hlcu = e->hl;
+    if (e->pix == 2) init_args(e, s, s.args16); else init_args(e, s, s.args8);
   }
   return e;
 }
 
-// common part of the two submit calls: `resident`: the planes are device memory and the results stay on the device
-static int submit_picture(kvz_cuda_ctu_enc *e, const uint8_t *y, const uint8_t *u, const uint8_t *v, int stride_y, int stride_c,
+}  // extern "C"
+
+// the search launch(es) of a submitted picture
+template <typename Pix> static int launch_search(kvz_cuda_ctu_enc *e, Slot &s, double lambda, double lambda_sqrt, int qp)
+{
+  KernelArgs<Pix> &a = args_of<Pix>(s);
+  cudaStream_t st = s.stream;
+  a.cfg = e->cfg;
+  a.cfg.lambda = lambda; a.cfg.lambda_sqrt = lambda_sqrt; a.cfg.qp = qp;
+  a.host_note = s.h_note;
+  a.seq = s.seq;
+  if (e->diag_launches) {
+    for (int d = 0; d < e->wl + 2 * (e->hl - 1); ++d) {
+      const int lo = d - (e->wl - 1) > 0 ? (d - (e->wl - 1) + 1) / 2 : 0, hi = d / 2 < e->hl - 1 ? d / 2 : e->hl - 1;
+      if (hi < lo) continue;
+      ctu_diag_kernel<Pix><<<hi - lo + 1, kThreads, e->smem, st>>>(a, d, lo);
+      e->launches.fetch_add(1, std::memory_order_relaxed);
+      kvzc::g_launches.fetch_add(1, std::memory_order_relaxed);
+    }
+  } else {
+    ctu_frame_kernel<Pix><<<e->grid, kThreads, e->smem, st>>>(a);
+    e->launches.fetch_add(1, std::memory_order_relaxed);
+    kvzc::g_launches.fetch_add(1, std::memory_order_relaxed);
+  }
+  return 0;
+}
+
+extern "C" {
+
+// common part of the two submit calls: `resident`: the planes are device memory and the results stay on the device.
+// Samples are uint8_t or uint16_t (cfg.bitdepth), strides in samples.
+static int submit_picture(kvz_cuda_ctu_enc *e, const void *y, const void *u, const void *v, int stride_y, int stride_c,
                           const uint8_t *ctx_init, double lambda, double lambda_sqrt, int qp, bool resident)
 {
   KVZC_ARG(e && y && u && v && ctx_init && stride_y >= e->cfg.width && stride_c >= e->cfg.width / 2);
@@ -356,43 +418,31 @@ static int submit_picture(kvz_cuda_ctu_enc *e, const uint8_t *y, const uint8_t *
   }
   Slot &s = e->slots[id];
   const int W = e->cfg.width, H = e->cfg.height;
-  const size_t ysz = (size_t)W * H, csz = ysz / 4;
+  const size_t px = (size_t)e->pix;
+  const size_t ysz = (size_t)W * H * px, csz = ysz / 4;           // bytes
+  const size_t wb = (size_t)W * px, sy = (size_t)stride_y * px, sc = (size_t)stride_c * px;
+  const uint8_t *yb = (const uint8_t *)y, *ub = (const uint8_t *)u, *vb = (const uint8_t *)v;
   cudaStream_t st = s.stream;
-  uint8_t *d_src = const_cast<uint8_t *>(s.args.F.src_y);
+  uint8_t *d_src = s.d_planes;        // (the source planes come first)
   if (resident) {
-    KVZC_CHECK(cudaMemcpy2DAsync(d_src, W, y, stride_y, W, H, cudaMemcpyDeviceToDevice, st));
-    KVZC_CHECK(cudaMemcpy2DAsync(d_src + ysz, W / 2, u, stride_c, W / 2, H / 2, cudaMemcpyDeviceToDevice, st));
-    KVZC_CHECK(cudaMemcpy2DAsync(d_src + ysz + csz, W / 2, v, stride_c, W / 2, H / 2, cudaMemcpyDeviceToDevice, st));
+    KVZC_CHECK(cudaMemcpy2DAsync(d_src, wb, yb, sy, wb, H, cudaMemcpyDeviceToDevice, st));
+    KVZC_CHECK(cudaMemcpy2DAsync(d_src + ysz, wb / 2, ub, sc, wb / 2, H / 2, cudaMemcpyDeviceToDevice, st));
+    KVZC_CHECK(cudaMemcpy2DAsync(d_src + ysz + csz, wb / 2, vb, sc, wb / 2, H / 2, cudaMemcpyDeviceToDevice, st));
   } else {
-    for (int r = 0; r < H; ++r) memcpy(s.h_src + (size_t)r * W, y + (size_t)r * stride_y, W);
+    for (int r = 0; r < H; ++r) memcpy(s.h_src + (size_t)r * wb, yb + (size_t)r * sy, wb);
     for (int r = 0; r < H / 2; ++r) {
-      memcpy(s.h_src + ysz + (size_t)r * (W / 2), u + (size_t)r * stride_c, W / 2);
-      memcpy(s.h_src + ysz + csz + (size_t)r * (W / 2), v + (size_t)r * stride_c, W / 2);
+      memcpy(s.h_src + ysz + (size_t)r * (wb / 2), ub + (size_t)r * sc, wb / 2);
+      memcpy(s.h_src + ysz + csz + (size_t)r * (wb / 2), vb + (size_t)r * sc, wb / 2);
     }
     KVZC_CHECK(cudaMemcpyAsync(d_src, s.h_src, e->plane_bytes, cudaMemcpyHostToDevice, st));
   }
   for (int r = 0; r < e->hl; ++r) { memcpy(s.h_row_ctx[r].ctx, ctx_init, CTX_COUNT); s.h_row_ctx[r].update = 0; memset(s.h_row_ctx[r].pad, 0, sizeof(s.h_row_ctx[r].pad)); }
-  s.args.cfg = e->cfg;
-  s.args.cfg.lambda = lambda; s.args.cfg.lambda_sqrt = lambda_sqrt; s.args.cfg.qp = qp;
   KVZC_CHECK(cudaMemcpyAsync(s.d_row_ctx, s.h_row_ctx, e->hl * sizeof(CabacState), cudaMemcpyHostToDevice, st));
   KVZC_CHECK(cudaMemsetAsync(s.d_cu, 0, (size_t)(e->wl * 16) * (e->hl * 16) * sizeof(CuRec), st));
   KVZC_CHECK(cudaMemsetAsync(s.d_sync, 0, (size_t)(e->hl + 2) * sizeof(int), st));
   s.seq += 1;
-  s.args.host_note = s.h_note;
-  s.args.seq = s.seq;
-  if (e->diag_launches) {
-    for (int d = 0; d < e->wl + 2 * (e->hl - 1); ++d) {
-      const int lo = d - (e->wl - 1) > 0 ? (d - (e->wl - 1) + 1) / 2 : 0, hi = d / 2 < e->hl - 1 ? d / 2 : e->hl - 1;
-      if (hi < lo) continue;
-      ctu_diag_kernel<<<hi - lo + 1, kThreads, e->smem, st>>>(s.args, d, lo);
-      e->launches.fetch_add(1, std::memory_order_relaxed);
-      kvzc::g_launches.fetch_add(1, std::memory_order_relaxed);
-    }
-  } else {
-    ctu_frame_kernel<<<e->grid, kThreads, e->smem, st>>>(s.args);
-    e->launches.fetch_add(1, std::memory_order_relaxed);
-    kvzc::g_launches.fetch_add(1, std::memory_order_relaxed);
-  }
+  if (e->pix == 2) launch_search<uint16_t>(e, s, lambda, lambda_sqrt, qp);
+  else launch_search<uint8_t>(e, s, lambda, lambda_sqrt, qp);
   if (e->diag_launches) KVZC_CHECK(cudaEventRecord(s.k1, st));
   KVZC_CHECK(cudaGetLastError());
   s.resident = resident;
@@ -415,7 +465,8 @@ static int finish_picture(kvz_cuda_ctu_enc *e, Slot &s)
     }
   }
   cudaStream_t st = s.stream;
-  ctu_sao_apply_kernel<<<e->wl * e->hl, kThreads, 0, st>>>(s.args);
+  if (e->pix == 2) ctu_sao_apply_kernel<uint16_t><<<e->wl * e->hl, kThreads, 0, st>>>(s.args16);
+  else ctu_sao_apply_kernel<uint8_t><<<e->wl * e->hl, kThreads, 0, st>>>(s.args8);
   e->launches.fetch_add(1, std::memory_order_relaxed);
   kvzc::g_launches.fetch_add(1, std::memory_order_relaxed);
   KVZC_CHECK(cudaGetLastError());
@@ -424,10 +475,10 @@ static int finish_picture(kvz_cuda_ctu_enc *e, Slot &s)
     KVZC_CHECK(cudaMemcpyAsync(s.h_cu, s.d_cu, (size_t)(e->wl * 16) * (e->hl * 16) * sizeof(CuRec), cudaMemcpyDeviceToHost, st));
     KVZC_CHECK(cudaMemcpyAsync(s.h_coeff, s.d_coeff, nctu * 6144 * sizeof(int16_t), cudaMemcpyDeviceToHost, st));
     KVZC_CHECK(cudaMemcpyAsync(s.h_sao, s.d_sao, nctu * 2 * sizeof(SaoRec), cudaMemcpyDeviceToHost, st));
-    KVZC_CHECK(cudaMemcpyAsync(s.h_out, s.args.F.out_y, e->plane_bytes, cudaMemcpyDeviceToHost, st));
+    KVZC_CHECK(cudaMemcpyAsync(s.h_out, s.d_planes + 2 * e->plane_bytes, e->plane_bytes, cudaMemcpyDeviceToHost, st));
     if (e->debug) {
       KVZC_CHECK(cudaMemcpyAsync(s.h_dbg_ctx, s.d_dbg_ctx, nctu * CTX_COUNT, cudaMemcpyDeviceToHost, st));
-      KVZC_CHECK(cudaMemcpyAsync(s.h_dbg, s.args.F.dbg_y, e->plane_bytes, cudaMemcpyDeviceToHost, st));
+      KVZC_CHECK(cudaMemcpyAsync(s.h_dbg, s.d_planes + 3 * e->plane_bytes, e->plane_bytes, cudaMemcpyDeviceToHost, st));
     }
   }
   KVZC_CHECK(cudaEventRecord(s.done, st));
@@ -456,7 +507,7 @@ int kvz_cuda_ctu_wait_device(kvz_cuda_ctu_enc *e, int slot, kvz_cuda_ctu_device_
   out->cu = (const kvz_cuda_ctu_cu *)s.d_cu;
   out->coeff = s.d_coeff;
   out->sao = (const kvz_cuda_ctu_sao *)s.d_sao;
-  out->rec = s.args.F.out_y;
+  out->rec = s.d_planes + 2 * e->plane_bytes;
   out->cu_stride = e->wl * 16;
   out->width_in_lcu = e->wl; out->height_in_lcu = e->hl;
   if (!e->diag_launches) out->search_kernel_ms = (float)((double)(s.h_note[2] - s.h_note[1]) * 1e-6);   // globaltimer ns of first / last CTA
@@ -468,7 +519,7 @@ int kvz_cuda_ctu_wait(kvz_cuda_ctu_enc *e, int slot, kvz_cuda_ctu_result *out)
   KVZC_ARG(e && out && slot >= 0 && slot < (int)e->slots.size() && e->slots[slot].state == 1);
   Slot &s = e->slots[slot];
   if (int rc = finish_picture(e, s)) return rc;
-  const size_t ysz = (size_t)e->cfg.width * e->cfg.height, csz = ysz / 4;
+  const size_t ysz = (size_t)e->cfg.width * e->cfg.height * e->pix, csz = ysz / 4;     // bytes
   memset(out, 0, sizeof(*out));
   out->cu = (const kvz_cuda_ctu_cu *)s.h_cu;
   out->cu_stride = e->wl * 16;

@@ -8,6 +8,7 @@ cd "$(dirname "$0")/.."
 FLAGS="-O1 -g -std=c++17 -fPIC -shared -ffp-contract=off -fsanitize=address,undefined -Wall -Wno-unused-function -Wno-unknown-pragmas"
 g++ $FLAGS -o /tmp/libkvzme_hostsim_asan.so tests/hostsim/me_hostsim.cpp
 g++ $FLAGS -o /tmp/libkvzctu_hostsim_asan.so tests/hostsim/ctu_hostsim.cpp
+g++ $FLAGS -o /tmp/libkvzctu_hostsim_10b_asan.so tests/hostsim/ctu_hostsim_10b.cpp
 ASAN=$(g++ -print-file-name=libasan.so)
 LD_PRELOAD=$ASAN ASAN_OPTIONS=detect_leaks=0 python - <<'PY'
 import ctypes as C, os, pathlib, subprocess, sys, tempfile
@@ -61,4 +62,16 @@ for (w, h, preset, qp, noisy) in [(264, 200, "veryslow", 22, False), (200, 136, 
                         "--threads", "2"], env=e, stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True, timeout=3000)
     issues = [ln for ln in r.stderr.splitlines() if "ERROR" in ln or "runtime error" in ln]
     print(f"CTU driver host build {w}x{h} {preset} q{qp}: rc {r.returncode}, active {'CTU search driver active' in r.stderr}, issues {len(issues)}")
+# the same at 10 bits (kvazaar_ctu_10b, genuine 10-bit content, the host build with both instantiations): the wider accumulators
+import test_ctu_driver_10bit as T10
+ctu10 = os.path.join(T.REF_DIR, "kvazaar_ctu_10b")
+for (w, h, preset, qp, noisy) in [(264, 200, "veryslow", 22, False), (200, 136, "medium", 27, True), (136, 72, "veryslow", 15, True),
+                                  (192, 64, "veryslow", 15, True), (72, 72, "placebo", 30, True)]:
+    clip = T10._clip(tmp, w, h, 1, noisy, 10)
+    e = dict(os.environ)
+    e.update({"KVZ_CTU_PROVIDER": "/tmp/libkvzctu_hostsim_10b_asan.so", "LD_PRELOAD": asan, "ASAN_OPTIONS": "detect_leaks=0:halt_on_error=0"})
+    r = subprocess.run([ctu10, "-i", clip, "--input-res", f"{w}x{h}", "--input-bitdepth", "10", "-o", str(tmp / "o.hevc"), "--preset", preset,
+                        "-q", str(qp), "-p", "1", "--threads", "2"], env=e, stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True, timeout=3000)
+    issues = [ln for ln in r.stderr.splitlines() if "ERROR" in ln or "runtime error" in ln]
+    print(f"CTU driver host build 10-bit {w}x{h} {preset} q{qp}: rc {r.returncode}, active {'CTU search driver active' in r.stderr}, issues {len(issues)}")
 PY

@@ -3,6 +3,7 @@
 `slots` pictures in flight.  With a `make PROF=1` build kvz_cuda_ctu_close prints the phase profile.
 
     python tools/ctu_devbench.py --res 1920x1080 --preset medium --frames 32 --slots 16
+    python tools/ctu_devbench.py --res 3840x2160 --preset veryslow --frames 8 --bitdepth 10    # Main 10 (uint16 samples)
 """
 import argparse
 import ctypes as C
@@ -23,7 +24,7 @@ class Config(C.Structure):
     _fields_ = [(n, C.c_int32) for n in (
         "width", "height", "qp", "rdo", "pu_depth_intra_min", "pu_depth_intra_max", "rdoq_enable", "rdoq_skip", "signhide_enable",
         "trskip_enable", "sao_type", "deblock_enable", "deblock_beta", "deblock_tc", "cu_split_termination", "intra_rdo_et",
-        "combine_intra_cus", "intra_chroma_search", "full_intra_search", "wpp", "pad")] + [("lambda_", C.c_double), ("lambda_sqrt", C.c_double)]
+        "combine_intra_cus", "intra_chroma_search", "full_intra_search", "wpp", "bitdepth")] + [("lambda_", C.c_double), ("lambda_sqrt", C.c_double)]
 
 
 class Result(C.Structure):
@@ -41,9 +42,10 @@ PRESETS = {
 }
 
 
-def make_config(w, h, preset, qp):
+def make_config(w, h, preset, qp, bitdepth=8):
     p = PRESETS[preset]
     c = Config()
+    c.bitdepth = bitdepth
     c.width, c.height, c.qp, c.rdo = w, h, qp, p["rdo"]
     c.pu_depth_intra_min, c.pu_depth_intra_max = p["pu"]
     c.rdoq_enable, c.rdoq_skip, c.signhide_enable, c.trskip_enable = p["rdoq"], 0, p["signhide"], p["trskip"]
@@ -62,11 +64,12 @@ def main():
     ap.add_argument("--frames", type=int, default=16)
     ap.add_argument("--slots", type=int, default=8)
     ap.add_argument("--distinct", type=int, default=4, help="distinct synthetic pictures (cycled)")
+    ap.add_argument("--bitdepth", type=int, default=8, choices=[8, 10])
     a = ap.parse_args()
     w, h = map(int, a.res.split("x"))
     qp = a.qp if a.qp is not None else {"ultrafast": 32, "medium": 27, "slow": 27, "veryslow": 22}[a.preset]
     import kvazaar_b200 as kb
-    from synth_yuv import synth_frame
+    from synth_yuv import frame_fn
     lib = C.CDLL(kb.LIB_PATH)
     lib.kvz_cuda_ctu_open.restype = C.c_void_p
     lib.kvz_cuda_ctu_open.argtypes = [C.POINTER(Config), C.c_int]
@@ -77,12 +80,12 @@ def main():
     lib.kvz_cuda_ctu_launches.restype = C.c_uint64
     lib.kvz_cuda_ctu_launches.argtypes = [C.c_void_p]
     lib.kvz_cuda_last_error.restype = C.c_char_p
-    cfg = make_config(w, h, a.preset, qp)
+    cfg = make_config(w, h, a.preset, qp, a.bitdepth)
     enc = lib.kvz_cuda_ctu_open(C.byref(cfg), a.slots)
     assert enc, lib.kvz_cuda_last_error()
     ctx = np.zeros(192, np.uint8)
     assert lib.kvz_cuda_cabac_ctx_init(qp, 2, ctx.ctypes.data_as(C.c_void_p)) == 0       # KVZ_SLICE_I = 2
-    frames = [synth_frame(w, h, 1234, i) for i in range(a.distinct)]
+    frames = [frame_fn(False, a.bitdepth)(w, h, 1234, i) for i in range(a.distinct)]
 
     def submit(i):
         f = frames[i % len(frames)]
@@ -110,7 +113,7 @@ def main():
         done += 1
     dt = time.perf_counter() - t0
     nctu = ((w + 63) // 64) * ((h + 63) // 64)
-    print(f"ctu_devbench {a.res} {a.preset} q{qp}: {a.frames} pictures, {a.slots} in flight: {a.frames / dt:.2f} pictures/s, "
+    print(f"ctu_devbench {a.res} {a.preset} q{qp} {a.bitdepth}-bit: {a.frames} pictures, {a.slots} in flight: {a.frames / dt:.2f} pictures/s, "
           f"{a.frames * nctu / dt:.0f} CTU/s, first picture after {first_latency * 1e3:.0f} ms, launches {lib.kvz_cuda_ctu_launches(enc)}", flush=True)
     lib.kvz_cuda_ctu_close(enc)
 
