@@ -29,16 +29,14 @@
 #define CTU_TID ((int)threadIdx.x)
 #define CTU_NT ((int)blockDim.x)
 #define CTU_SYNC() __syncthreads()
-// a "team" is the first warp of the CTA: used by the algorithms with a serial spine (RDOQ) so that their inner
-// synchronisation is a warp barrier; the rest of the CTA waits at the next CTA barrier
+// the algorithms with a serial spine (RDOQ) run on at most one warp of a team, so that their inner synchronisation is a
+// warp barrier; the rest of the CTA waits at the next CTA barrier
 #define CTU_TEAM_N 32
-#define CTU_TEAM_SYNC() __syncwarp()
 #else
 #define CTU_TID 0
 #define CTU_NT 1
 #define CTU_SYNC() ((void)0)
 #define CTU_TEAM_N 1
-#define CTU_TEAM_SYNC() ((void)0)
 #endif
 // The leader is lane 0 of ONE of the CTA's warps, chosen per CTA (first word of the CTA's shared memory, set by the kernel):
 // the CTAs that share an SM get different leader warps, so their serial sections run on different SM sub-partitions
@@ -63,14 +61,18 @@ extern __shared__ __align__(16) unsigned char ctu_smem_raw[];
 #endif
 
 // Phase profile (diagnostic build, make PROF=1): cycles of the leader thread per phase, summed over all CTUs.
-enum { PR_LOAD, PR_SEARCH, PR_STORE, PR_DEBLOCK, PR_SAO, PR_TRACK, PR_REFS, PR_SATD, PR_REPLAY, PR_PREDICT, PR_QRES, PR_FWD, PR_RDOQ, PR_QUANT,
+// PR_QRES / PR_QRES4: transform-unit job batches with a unit larger than 4x4 / of 4x4 units only.  PR_COEFFCOST: the
+// coefficient bits of the RDO candidates' jobs that ran on the leader's team (a part of their batch's time).
+enum { PR_LOAD, PR_SEARCH, PR_STORE, PR_DEBLOCK, PR_SAO, PR_TRACK, PR_REFS, PR_SATD, PR_REPLAY, PR_PREDICT, PR_QRES, PR_QRES4, PR_FWD, PR_RDOQ, PR_QUANT,
        PR_INV, PR_SSD, PR_COST, PR_COPY, PR_COEFFCOST, PR_WAIT, PR_CHROMA, PR_RDO_LOOP, PR_WRITEBACK, PR_N };
 #if defined(KVZ_CTU_PROF) && defined(__CUDA_ARCH__)
 #define PROF_T0(id) const long long prof_t0_##id = clock64()
 #define PROF_ADD(S, id) do { if (CTU_TID == CTU_LEADER_TID) (S)->prof[id] += clock64() - prof_t0_##id; } while (0)
+#define PROF_ADD_AS(S, id, as) do { if (CTU_TID == CTU_LEADER_TID) (S)->prof[as] += clock64() - prof_t0_##id; } while (0)
 #else
 #define PROF_T0(id) ((void)0)
 #define PROF_ADD(S, id) ((void)0)
+#define PROF_ADD_AS(S, id, as) ((void)0)
 #endif
 
 namespace kvzctu {

@@ -49,21 +49,28 @@ template <typename Pix> struct IntraRefs {                  // kvz_intra_referen
 };
 
 // ------------------------------------------------------------------------------------------------ teams
-// A team is the group of threads that evaluates one transform unit: the whole CTA for 32x32 units, one warp for the
-// smaller ones (several units -- colour planes, RDO candidates -- are then evaluated side by side, one per warp).
-struct Team { int tid, nt, warp; };
+// A team is the group of threads that evaluates one transform unit: the whole CTA for 32x32 units, one warp for 8x8 and
+// 16x16 units, half a warp for 4x4 units (several units -- colour planes, RDO candidates -- are then evaluated side by
+// side, one per team).  A 4x4 unit has 16 coefficients: on a whole warp every data-parallel stage would leave half the
+// lanes idle, and its serial sections (RDOQ's walk, the coefficient bits) run on one lane either way.  The two halves
+// of a warp run the same code on different units, mostly in lockstep.  `mask`: the lanes of a warp team (tsync).
+struct Team { int tid, nt, warp; unsigned mask; };
 #if defined(__CUDA_ARCH__)
-CTU_FN Team team_cta() { Team t = { (int)threadIdx.x, (int)blockDim.x, 0 }; return t; }
-CTU_FN Team team_warp() { Team t = { (int)(threadIdx.x & 31), 32, 1 }; return t; }
-CTU_FN void tsync(const Team &t) { if (t.warp) __syncwarp(); else __syncthreads(); }
+CTU_FN Team team_cta() { Team t = { (int)threadIdx.x, (int)blockDim.x, 0, 0xffffffffu }; return t; }
+CTU_FN Team team_warp() { Team t = { (int)(threadIdx.x & 31), 32, 1, 0xffffffffu }; return t; }
+CTU_FN Team team_half() { Team t = { (int)(threadIdx.x & 15), 16, 1, 0xffffu << (threadIdx.x & 16) }; return t; }
+CTU_FN void tsync(const Team &t) { if (t.warp) __syncwarp(t.mask); else __syncthreads(); }
 #define CTU_NWARPS ((int)(blockDim.x >> 5))
 #define CTU_WARP ((int)(threadIdx.x >> 5))
+#define CTU_HALF ((int)(threadIdx.x >> 4))
 #else
-CTU_FN Team team_cta() { Team t = { 0, 1, 0 }; return t; }
-CTU_FN Team team_warp() { Team t = { 0, 1, 1 }; return t; }
+CTU_FN Team team_cta() { Team t = { 0, 1, 0, 0 }; return t; }
+CTU_FN Team team_warp() { Team t = { 0, 1, 1, 0 }; return t; }
+CTU_FN Team team_half() { Team t = { 0, 1, 1, 0 }; return t; }
 CTU_FN void tsync(const Team &) {}
 #define CTU_NWARPS 1
 #define CTU_WARP 0
+#define CTU_HALF 0
 #endif
 
 // All tables the search reads, compact, in shared memory (copied from the host-built CtuTables once per CTU): the serial
@@ -78,8 +85,8 @@ struct SmTables {
   int8_t tr4[16], tr8[64], tr16[256], tr32[1024], dst4[16];
   uint8_t sig_ctx4[16], group_idx[32], min_in_group[10];
   uint8_t pad[6];
-  // not a table: the absolute levels of the coefficient group being counted, one row per warp (a thread-local array
-  // indexed at run time would live in local memory, behind the 34 KB of L1 three CTAs share)
+  // not a table: the absolute levels of the coefficient group being counted, one row per half-warp, the smallest team
+  // (a thread-local array indexed at run time would live in local memory, behind the 34 KB of L1 three CTAs share)
   mutable int32_t abs_scratch[8][16];
 };
 CTU_FN const uint16_t *sm_scan(const SmTables *t, int scan_idx, int l)      // l = log2n - 2
@@ -765,19 +772,23 @@ template <typename Pix> CTU_FN_NOINLINE void rdoq_sign_hiding(const TuS<Pix> &tu
   }
 }
 
+// RDOQ runs on the first nl = rdoq_lanes() threads of a team (the first warp of a CTA team), whose lanes are `mask`
+CTU_FN int rdoq_lanes(const Team &t) { return t.nt < CTU_TEAM_N ? t.nt : CTU_TEAM_N; }
 #if defined(__CUDA_ARCH__)
-CTU_FN int team_max(int v) { for (int o = 16; o > 0; o >>= 1) v = max(v, __shfl_xor_sync(0xffffffffu, v, o)); return v; }
-CTU_FN int team_sum(int v) { for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o); return v; }
+CTU_FN void rq_sync(unsigned mask) { __syncwarp(mask); }
+CTU_FN int team_max(int v, unsigned mask, int nl) { for (int o = nl >> 1; o > 0; o >>= 1) v = max(v, __shfl_xor_sync(mask, v, o)); return v; }
+CTU_FN int team_sum(int v, unsigned mask, int nl) { for (int o = nl >> 1; o > 0; o >>= 1) v += __shfl_xor_sync(mask, v, o); return v; }
 #else
-CTU_FN int team_max(int v) { return v; }
-CTU_FN int team_sum(int v) { return v; }
+CTU_FN void rq_sync(unsigned) {}
+CTU_FN int team_max(int v, unsigned, int) { return v; }
+CTU_FN int team_sum(int v, unsigned, int) { return v; }
 #endif
 
-// kvz_rdoq for one TU, executed by one team (the first warp): coef = tu->b, levels to tu->q.  `cabac` = the models of
-// state->cabac (NOT the search copy: rdo.c:665).  type 0 luma / 2 chroma; tr_depth as in quant-generic.c:237-238.
+// kvz_rdoq for one TU, executed by the RDOQ lanes of a team (lane < nl): coef = tu->b, levels to tu->q.  `cabac` = the
+// models of state->cabac (NOT the search copy: rdo.c:665).  type 0 luma / 2 chroma; tr_depth as in quant-generic.c:237-238.
 template <int L2N, typename Pix>
 CTU_FN_NOINLINE void rdoq_team(const SmTables *T, const SmTables *tb, const CtuConfig *cfg, const uint8_t *cabac, const TuS<Pix> &tu, int log2n_rt, int type,
-                      int scan_idx, int tr_depth, int lane)
+                      int scan_idx, int tr_depth, int lane, int nl, unsigned mask)
 {
   const int log2n = L2N ? L2N : log2n_rt;
   const int16_t *coef = tu.b();
@@ -816,17 +827,17 @@ CTU_FN_NOINLINE void rdoq_team(const SmTables *T, const SmTables *tb, const CtuC
 
   int my_last = -1;
   #pragma unroll 1
-  for (int sp = lane; sp < nn; sp += CTU_TEAM_N) {
+  for (int sp = lane; sp < nn; sp += nl) {
     const int ld = imin(iabs((int)coef[blk_of[sp]]) * qc, 0x7FFFFFFF - half);
     if (((ld + half) >> q_bits) > 0) my_last = sp;
   }
-  const int last_scanpos = team_max(my_last);
-  CTU_TEAM_SYNC();
+  const int last_scanpos = team_max(my_last, mask, nl);
+  rq_sync(mask);
   #pragma unroll 1
-  for (int sp = lane; sp < nn; sp += CTU_TEAM_N) if (sp > last_scanpos) q[blk_of[sp]] = 0;
-  if (last_scanpos < 0) { CTU_TEAM_SYNC(); return; }
+  for (int sp = lane; sp < nn; sp += nl) if (sp > last_scanpos) q[blk_of[sp]] = 0;
+  if (last_scanpos < 0) { rq_sync(mask); return; }
   #pragma unroll 1
-  for (int g = lane; g < nn / 16; g += CTU_TEAM_N) { s_cg_flag[g] = 0; s_cg_sig_cost[g] = 0; }
+  for (int g = lane; g < nn / 16; g += nl) { s_cg_flag[g] = 0; s_cg_sig_cost[g] = 0; }
   if (lane == 0) {
     if (SH) s_sig_inc[blk_of[last_scanpos]] = 0;
     const int cb = log2n - 2;
@@ -841,7 +852,7 @@ CTU_FN_NOINLINE void rdoq_team(const SmTables *T, const SmTables *tb, const CtuC
     }
     s.last_x_bits[ctx] = bx; s.last_y_bits[ctx] = by;
   }
-  CTU_TEAM_SYNC();
+  rq_sync(mask);
 
   const int cg_last = last_scanpos >> 4;
   const int cgs_side = n >> 2;
@@ -858,7 +869,7 @@ CTU_FN_NOINLINE void rdoq_team(const SmTables *T, const SmTables *tb, const CtuC
     const int lower = (cgy < cgs_side - 1) ? (s_cg_flag[(cgy + 1) * cgs_side + cgx] != 0) : 0;
     const int pattern = (n == 4) ? -1 : right + (lower << 1);
     #pragma unroll 1
-    for (int k = lane; k < 16; k += CTU_TEAM_N) {
+    for (int k = lane; k < 16; k += nl) {
       const int sp = (cg << 4) + k;
       uint8_t fl = 0;
       if (sp <= last_scanpos) {
@@ -887,7 +898,7 @@ CTU_FN_NOINLINE void rdoq_team(const SmTables *T, const SmTables *tb, const CtuC
       }
       s.prep_flags[k] = fl;
     }
-    CTU_TEAM_SYNC();
+    rq_sync(mask);
 
     if (lane == 0) {
       double st_coded = 0, st_uncoded = 0, st_sig = 0, st_sig0 = 0;
@@ -1000,7 +1011,7 @@ CTU_FN_NOINLINE void rdoq_team(const SmTables *T, const SmTables *tb, const CtuC
       }
       s_cg_nz[cg] = (uint16_t)nz_mask;
     }
-    CTU_TEAM_SYNC();
+    rq_sync(mask);
   }
 
   if (lane == 0) {
@@ -1039,12 +1050,12 @@ CTU_FN_NOINLINE void rdoq_team(const SmTables *T, const SmTables *tb, const CtuC
     }
     s.best_last_p1 = best_last_p1;
   }
-  CTU_TEAM_SYNC();
+  rq_sync(mask);
 
   const int best_last_p1 = s.best_last_p1;
   int abs_sum = 0;
   #pragma unroll 1
-  for (int sp = lane; sp <= last_scanpos; sp += CTU_TEAM_N) {
+  for (int sp = lane; sp <= last_scanpos; sp += nl) {
     const int blk = blk_of[sp];
     if (sp < best_last_p1) {
       const int level = q[blk];
@@ -1055,11 +1066,11 @@ CTU_FN_NOINLINE void rdoq_team(const SmTables *T, const SmTables *tb, const CtuC
     }
   }
   if (SH) {
-    abs_sum = team_sum(abs_sum);
-    CTU_TEAM_SYNC();
+    abs_sum = team_sum(abs_sum, mask, nl);
+    rq_sync(mask);
     if (lane == 0 && abs_sum >= 2) rdoq_sign_hiding(tu, blk_of, lambda, qp_scaled, best_last_p1, coef, q);
   }
-  CTU_TEAM_SYNC();
+  rq_sync(mask);
 }
 
 // ------------------------------------------------------------------------------------------------ CABAC bins (leader only)
@@ -1144,7 +1155,7 @@ CTU_FN_NOINLINE double coeff_cost_serial(const SmTables *T, const SmTables *tb, 
   int scan_pos_sig = scan_last;
   for (int i = cg_last; i >= 0; --i) {
     const int sub_pos = i << 4;
-    int32_t *abs_coeff = tb->abs_scratch[CTU_WARP & 7];
+    int32_t *abs_coeff = tb->abs_scratch[CTU_HALF & 7];
     const int cg_blk = scan_cg[i];
     const int cgy = cg_blk / side, cgx = cg_blk - cgy * side;
     int last_nz = -1, first_nz = 16, num_nz = 0, rice = 0;
@@ -1251,7 +1262,8 @@ CTU_FN_NOINLINE void tu_core_t(const Team &tm, const SmTables *T, const SmTables
   }
   const int type = color == 0 ? 0 : 2;
   if (cfg->rdoq_enable && (n > 4 || !cfg->rdoq_skip)) {
-    if (tm.tid < CTU_TEAM_N) rdoq_team<L2N>(T, tb, cfg, cabac0, tu, log2n, type, j.scan_idx, j.rdoq_tr_depth, tm.tid);
+    const int nl = rdoq_lanes(tm);
+    if (tm.tid < nl) rdoq_team<L2N>(T, tb, cfg, cabac0, tu, log2n, type, j.scan_idx, j.rdoq_tr_depth, tm.tid, nl, tm.mask);
     tsync(tm);
   } else {
     quant_block(tm, T, cfg, tu, n, type, j.scan_idx);

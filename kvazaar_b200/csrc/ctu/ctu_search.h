@@ -218,13 +218,18 @@ template <typename Pix> CTU_FN double coeff_cost_of_unit(const CtxT<Pix> &c, Cab
   return coeff_cost_serial(&c.S->tb, &c.S->tb, c.cfg, sc, co, log2n, type, scan, 0, mask);
 }
 
-// Runs `ntasks` independent transform-unit jobs whose largest unit has nn coefficients: one warp per job when four
-// scratch slots fit the arena, otherwise the whole CTA job after job.  f(team, slot base, task) must synchronise
-// with tsync(team) only.
+// Runs `ntasks` independent transform-unit jobs whose largest unit has nn coefficients: one half-warp per job when all
+// units are 4x4, one warp per job when four scratch slots fit the arena, otherwise the whole CTA job after job.
+// f(team, slot base, task) must synchronise with tsync(team) only.  Tasks 2i and 2i + 1 run on the two halves of one
+// warp: callers put units that take the same path through the job next to each other.
 template <typename Pix, class F> CTU_FN void for_tu_tasks(const CtxT<Pix> &c, int ntasks, int nn, F f)
 {
   CTU_SYNC();
-  if (CTU_NWARPS > 1 && CTU_NWARPS * tu_scratch_bytes<Pix>(nn) <= CTU_ARENA_BYTES) {
+  if (nn == 16 && CTU_NWARPS > 1 && 2 * CTU_NWARPS * tu_scratch_bytes<Pix>(nn) <= CTU_ARENA_BYTES) {
+    const Team tm = team_half();
+    unsigned char *slot = c.S->arena + (size_t)CTU_HALF * tu_scratch_bytes<Pix>(nn);
+    for (int t = CTU_HALF; t < ntasks; t += 2 * CTU_NWARPS) f(tm, slot, t);
+  } else if (CTU_NWARPS > 1 && CTU_NWARPS * tu_scratch_bytes<Pix>(nn) <= CTU_ARENA_BYTES) {
     const Team tm = team_warp();
     unsigned char *slot = c.S->arena + (size_t)CTU_WARP * tu_scratch_bytes<Pix>(nn);
     for (int t = CTU_WARP; t < ntasks; t += CTU_NWARPS) f(tm, slot, t);
@@ -293,7 +298,7 @@ template <typename Pix> CTU_FN_NOINLINE void intra_recon_leaf(const CtxT<Pix> &c
     }
     tsync(tm);
   });
-  PROF_ADD(S, PR_QRES);
+  PROF_ADD_AS(S, PR_QRES, tu_log2(depth, first) == 2 ? PR_QRES4 : PR_QRES);
   CTU_LEADER {
     const bool ts_branch = depth == 4 && c.cfg->trskip_enable;       // 4x4 luma units only (transform.c:366)
     for (int col = first; col <= last; ++col) {
@@ -770,11 +775,13 @@ template <typename Pix> CTU_FN_NOINLINE void search_cu_intra(const CtxT<Pix> &c,
         r->ssd = fx->ssd; r->has = fx->has; r->tr_skip = ts;
         r->cg_mask = (uint64_t)fx->cg_mask[0] | ((uint64_t)fx->cg_mask[1] << 32);
         // coefficient bits of kvz_cu_rd_cost_luma / _chroma: the search models are not adapted here (update == 0)
+        PROF_T0(PR_COEFFCOST);
         r->bits = fx->has ? coeff_cost_serial(&c.S->tb, &S->tb, cfg, &S->sc, tu.q(), log2n, col ? 2 : 0, j.scan_idx, 0, r->cg_mask) : 0.0;
+        PROF_ADD(S, PR_COEFFCOST);
       }
       tsync(tm);
     });
-    PROF_ADD(S, PR_QRES);
+    PROF_ADD_AS(S, PR_QRES, log2w == 2 ? PR_QRES4 : PR_QRES);
     PROF_T0(PR_COST);
     int checked = ncand;
     CTU_LEADER {
