@@ -61,10 +61,12 @@ extern __shared__ __align__(16) unsigned char ctu_smem_raw[];
 #endif
 
 // Phase profile (diagnostic build, make PROF=1): cycles of the leader thread per phase, summed over all CTUs.
-// PR_QRES / PR_QRES4: transform-unit job batches with a unit larger than 4x4 / of 4x4 units only.  PR_COEFFCOST: the
-// coefficient bits of the RDO candidates' jobs that ran on the leader's team (a part of their batch's time).
-enum { PR_LOAD, PR_SEARCH, PR_STORE, PR_DEBLOCK, PR_SAO, PR_TRACK, PR_REFS, PR_SATD, PR_REPLAY, PR_PREDICT, PR_QRES, PR_QRES4, PR_FWD, PR_RDOQ, PR_QUANT,
-       PR_INV, PR_SSD, PR_COST, PR_COPY, PR_COEFFCOST, PR_WAIT, PR_CHROMA, PR_RDO_LOOP, PR_WRITEBACK, PR_N };
+// PR_QRES4 .. PR_QRES32: transform-unit job batches whose largest unit is 4x4, 8x8, 16x16, 32x32 (pr_qres_of).
+// PR_COEFFCOST: the coefficient bits of the RDO candidates' jobs that ran on the leader's team (a part of their batch's
+// time).
+enum { PR_LOAD, PR_SEARCH, PR_STORE, PR_DEBLOCK, PR_SAO, PR_TRACK, PR_REFS, PR_SATD, PR_REPLAY, PR_QRES4, PR_QRES8, PR_QRES16, PR_QRES32,
+       PR_COST, PR_COPY, PR_COEFFCOST, PR_WAIT, PR_CHROMA, PR_RDO_LOOP, PR_WRITEBACK, PR_N };
+#define pr_qres_of(log2n) (PR_QRES4 + (log2n) - 2)
 #if defined(KVZ_CTU_PROF) && defined(__CUDA_ARCH__)
 #define PROF_T0(id) const long long prof_t0_##id = clock64()
 #define PROF_ADD(S, id) do { if (CTU_TID == CTU_LEADER_TID) (S)->prof[id] += clock64() - prof_t0_##id; } while (0)

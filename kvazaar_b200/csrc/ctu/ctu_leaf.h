@@ -50,8 +50,8 @@ template <typename Pix> struct IntraRefs {                  // kvz_intra_referen
 
 // ------------------------------------------------------------------------------------------------ teams
 // A team is the group of threads that evaluates one transform unit: the whole CTA for 32x32 units, one warp for 8x8 and
-// 16x16 units, half a warp for 4x4 units (several units -- colour planes, RDO candidates -- are then evaluated side by
-// side, one per team).  A 4x4 unit has 16 coefficients: on a whole warp every data-parallel stage would leave half the
+// 16x16 units, half a warp for the 4x4 units of batches of 4x4 units only (several units -- colour planes, RDO
+// candidates -- are then evaluated side by side, one per team; see for_tu_tasks).  A 4x4 unit has 16 coefficients: on a whole warp every data-parallel stage would leave half the
 // lanes idle, and its serial sections (RDOQ's walk, the coefficient bits) run on one lane either way.  The two halves
 // of a warp run the same code on different units, mostly in lockstep.  `mask`: the lanes of a warp team (tsync).
 struct Team { int tid, nt, warp; unsigned mask; };
@@ -172,7 +172,8 @@ template <typename Pix> CTU_FN TuS<Pix> tu_scratch(unsigned char *arena, int nn,
   return t;
 }
 // One 32x32 unit, or four units of up to 16x16 side by side.  With 16-bit samples four 16x16 units need 42 176 bytes:
-// the arena keeps its size (three CTAs per SM) and for_tu_tasks runs such units one after another on the whole CTA.
+// the arena keeps its size (three CTAs per SM) and for_tu_tasks runs batches with such units one after another on the
+// whole CTA.
 #define CTU_ARENA_BYTES 40960
 
 // ------------------------------------------------------------------------------------------------ pixel planes

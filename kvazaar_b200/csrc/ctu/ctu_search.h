@@ -17,7 +17,7 @@
 // operation order (the build uses -fmad=false), same CABAC model adaptation.  What differs is how the work is laid
 // out: the rough search evaluates the SATD of all 35 modes in one data-parallel phase and then replays the reference's
 // halving search on the table; the RDO candidates of search_intra_rdo and the colours of a CU are independent
-// transform-unit jobs that run one per warp (for_tu_tasks) with private reconstructions, and only SSD / cbf / exact
+// transform-unit jobs that run on teams sized to their units (for_tu_tasks) with private reconstructions, and only SSD / cbf / exact
 // coefficient bits come back to the leader, which assembles the costs in the reference's order; each job keeps its
 // reconstruction and levels in CtuWork, and the winner's are written back where the reference reconstructs the chosen
 // mode once more; the cost walks that adapt the context models stay serial on the leader.
@@ -218,24 +218,59 @@ template <typename Pix> CTU_FN double coeff_cost_of_unit(const CtxT<Pix> &c, Cab
   return coeff_cost_serial(&c.S->tb, &c.S->tb, c.cfg, sc, co, log2n, type, scan, 0, mask);
 }
 
-// Runs `ntasks` independent transform-unit jobs whose largest unit has nn coefficients: one half-warp per job when all
-// units are 4x4, one warp per job when four scratch slots fit the arena, otherwise the whole CTA job after job.
-// f(team, slot base, task) must synchronise with tsync(team) only.  Tasks 2i and 2i + 1 run on the two halves of one
-// warp: callers put units that take the same path through the job next to each other.
-template <typename Pix, class F> CTU_FN void for_tu_tasks(const CtxT<Pix> &c, int ntasks, int nn, F f)
+// The class of a transform-unit task for for_tu_tasks: its unit's log2 side (bits 0..2) and luma or chroma.
+CTU_FN int tu_class(int log2n, int color) { return log2n | (color ? 8 : 0); }
+
+// Runs `ntasks` (at most 32) independent transform-unit jobs; class_of(t) is tu_class() of task t.  32x32 units run
+// on the whole CTA, one after another.  In a batch of 4x4 units only, two consecutive tasks of the same class run on
+// the two halves of one warp, so that both halves take the same path through the job (callers put such units next to
+// each other: two luma units, or the U and V units of one candidate); a unit without such a neighbour leaves the other
+// half idle.  Every other unit up to 16x16 runs on one warp, when four slots of the batch's largest such unit fit the
+// arena (not 16x16 at 16-bit samples: then on the whole CTA as well).  The warp jobs -- a unit, or a pair of 4x4 units
+// -- go to the warps in turn.  (Half-warp teams for the 4x4 and 8x8 units of mixed batches were measured slower: the
+// two halves' serial sections -- RDOQ's walk, the coefficient bits -- diverge and run one after the other, so a pair
+// takes about as long as two units on whole warps.)  f(team, slot base, task) must synchronise with tsync(team) only.
+template <typename Pix, class K, class F> CTU_FN void for_tu_tasks(const CtxT<Pix> &c, int ntasks, K class_of, F f)
 {
   CTU_SYNC();
-  if (nn == 16 && CTU_NWARPS > 1 && 2 * CTU_NWARPS * tu_scratch_bytes<Pix>(nn) <= CTU_ARENA_BYTES) {
-    const Team tm = team_half();
-    unsigned char *slot = c.S->arena + (size_t)CTU_HALF * tu_scratch_bytes<Pix>(nn);
-    for (int t = CTU_HALF; t < ntasks; t += 2 * CTU_NWARPS) f(tm, slot, t);
-  } else if (CTU_NWARPS > 1 && CTU_NWARPS * tu_scratch_bytes<Pix>(nn) <= CTU_ARENA_BYTES) {
-    const Team tm = team_warp();
-    unsigned char *slot = c.S->arena + (size_t)CTU_WARP * tu_scratch_bytes<Pix>(nn);
-    for (int t = CTU_WARP; t < ntasks; t += CTU_NWARPS) f(tm, slot, t);
-  } else {
+  const int nw = CTU_NWARPS;
+  int lmax = 2;                     // the largest unit up to 16x16
+  bool only4 = true;
+  for (int t = 0; t < ntasks; ++t) {
+    const int l = class_of(t) & 7;
+    if (l != 2) only4 = false;
+    if (l <= 4) lmax = imax(lmax, l);
+  }
+  const bool halves = nw > 1 && only4 && nw * 2 * tu_scratch_bytes<Pix>(16) <= CTU_ARENA_BYTES;
+  const int warp_bytes = halves ? 2 * tu_scratch_bytes<Pix>(16) : tu_scratch_bytes<Pix>(1 << (2 * lmax));
+  const bool warps = nw > 1 && nw * warp_bytes <= CTU_ARENA_BYTES;
+  // the tasks of the CTA, of this thread's warp as a whole, of its half-warp (bit t: task t)
+  unsigned cta = 0, whole = 0, half = 0;
+  int job = 0;                      // warp job `job` runs on warp job % nw
+  for (int t = 0; t < ntasks; ++t) {
+    if ((class_of(t) & 7) > 4 || !warps) { cta |= 1u << t; continue; }
+    const bool pair = halves && t + 1 < ntasks && class_of(t + 1) == class_of(t);
+    if (job++ % nw == CTU_WARP) {
+      if (!halves) whole |= 1u << t;
+      else if (!(CTU_HALF & 1)) half |= 1u << t;
+      else if (pair) half |= 2u << t;
+    }
+    if (pair) ++t;
+  }
+  if (cta) {
     const Team tm = team_cta();
-    for (int t = 0; t < ntasks; ++t) f(tm, c.S->arena, t);
+    for (int t = 0; t < ntasks; ++t) if ((cta >> t) & 1) f(tm, c.S->arena, t);
+    CTU_SYNC();
+  }
+  unsigned char *base = c.S->arena + (size_t)CTU_WARP * warp_bytes;
+  if (whole) {
+    const Team tm = team_warp();
+    for (int t = 0; t < ntasks; ++t) if ((whole >> t) & 1) f(tm, base, t);
+  }
+  if (half) {
+    const Team tm = team_half();
+    unsigned char *slot = base + (size_t)(CTU_HALF & 1) * tu_scratch_bytes<Pix>(16);
+    for (int t = 0; t < ntasks; ++t) if ((half >> t) & 1) f(tm, slot, t);
   }
   CTU_SYNC();
 }
@@ -264,8 +299,9 @@ template <typename Pix> CTU_FN_NOINLINE void intra_recon_leaf(const CtxT<Pix> &c
   PROF_ADD(S, PR_REFS);
   // cur_pu of quantize_tr_residual: the RDOQ context selector reads its depths before the cbf bits change
   const int rdoq_tr_depth = (int)cur_cu->tr_depth - (int)cur_cu->depth + (cur_cu->part_size == SIZE_NxN ? 1 : 0);
-  PROF_T0(PR_QRES);
-  for_tu_tasks(c, last - first + 1, 1 << (2 * tu_log2(depth, first)), [&](const Team &tm, unsigned char *slot, int t) {
+  PROF_T0(PR_QRES4);
+  // tasks luma, U, V: U and V share a warp when their units are 4x4
+  for_tu_tasks(c, last - first + 1, [&](int t) { return tu_class(tu_log2(depth, first + t), first + t); }, [&](const Team &tm, unsigned char *slot, int t) {
     const int col = first + t;
     const int log2n = tu_log2(depth, col), n = 1 << log2n;
     const TuS<Pix> tu = tu_at<Pix>(slot, n * n);
@@ -298,7 +334,7 @@ template <typename Pix> CTU_FN_NOINLINE void intra_recon_leaf(const CtxT<Pix> &c
     }
     tsync(tm);
   });
-  PROF_ADD_AS(S, PR_QRES, tu_log2(depth, first) == 2 ? PR_QRES4 : PR_QRES);
+  PROF_ADD_AS(S, PR_QRES4, pr_qres_of(tu_log2(depth, first)));
   CTU_LEADER {
     const bool ts_branch = depth == 4 && c.cfg->trskip_enable;       // 4x4 luma units only (transform.c:366)
     for (int col = first; col <= last; ++col) {
@@ -742,16 +778,20 @@ template <typename Pix> CTU_FN_NOINLINE void search_cu_intra(const CtxT<Pix> &c,
     // cbf context and the cbf bits collected below.
     const int ncand = S->n_modes;
     const int rdoq_tr_depth = depth == 4 ? 1 : 0;
-    PROF_T0(PR_QRES);
+    PROF_T0(PR_QRES4);
     // 4x4 luma units with transform skip enabled: the two alternatives of kvz_quantize_residual_trskip are jobs of their
     // own (better balance over the warps), the leader picks below; the pick's coefficient bits are the ones its luma
     // cost needs (same call: rdo.c:251-258 codes tr_skip as 0), so they are not computed a third time
     const bool ts_split = depth == 4 && cfg->trskip_enable;
     const int nluma = ts_split ? 2 : 1;
-    const int per_cand = nluma + (np - 1);
-    for_tu_tasks(c, ncand * per_cand, 1 << (2 * log2w), [&](const Team &tm, unsigned char *slot, int t) {
-      const int cand = t / per_cand, k = t - cand * per_cand;
-      const int col = k < nluma ? 0 : 1 + (k - nluma);
+    // tasks: the luma units of all candidates (k: the transform-skip alternative), then (U, V) of each candidate, so
+    // that the two halves of a warp get two luma units or the two chroma units of one candidate
+    const int ntl = ncand * nluma;
+    for_tu_tasks(c, ntl + ncand * (np - 1), [&](int t) { return t < ntl ? tu_class(log2w, 0) : tu_class(tu_log2(depth, 1), 1); },
+                 [&](const Team &tm, unsigned char *slot, int t) {
+      const int cand = t < ntl ? t / nluma : (t - ntl) >> 1;
+      const int k = t < ntl ? t - cand * nluma : 0;
+      const int col = t < ntl ? 0 : 1 + ((t - ntl) & 1);
       const int mode = S->modes[cand];
       const int log2n = tu_log2(depth, col), n = 1 << log2n;
       const TuS<Pix> tu = tu_at<Pix>(slot, n * n);
@@ -781,7 +821,7 @@ template <typename Pix> CTU_FN_NOINLINE void search_cu_intra(const CtxT<Pix> &c,
       }
       tsync(tm);
     });
-    PROF_ADD_AS(S, PR_QRES, log2w == 2 ? PR_QRES4 : PR_QRES);
+    PROF_ADD_AS(S, PR_QRES4, pr_qres_of(log2w));
     PROF_T0(PR_COST);
     int checked = ncand;
     CTU_LEADER {

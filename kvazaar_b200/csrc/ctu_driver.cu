@@ -248,8 +248,9 @@ void kvz_cuda_ctu_close(kvz_cuda_ctu_enc *e)
   }
 #if defined(KVZ_CTU_PROF)
   if (e->d_prof) {
-    static const char *names[PR_N + 1] = { "load", "search(total)", "store", "deblock", "sao", "track", "  refs", "  satd(rough)", "  replay", "  predict", "  quantize_residual(>4x4 batches)",
-      "  quantize_residual(4x4 batches)", "    fwd", "    rdoq", "    quant", "    inv+rec", "  ssd", "  cost(leader)", "  copies",
+    static const char *names[PR_N + 1] = { "load", "search(total)", "store", "deblock", "sao", "track", "  refs", "  satd(rough)", "  replay",
+      "  quantize_residual(4x4 batches)", "  quantize_residual(8x8 batches)", "  quantize_residual(16x16 batches)",
+      "  quantize_residual(32x32 batches)", "  cost(leader)", "  copies",
       "    rdo job coeff bits(leader's team)", "wait(deps)", "  chroma search(total)", "  rdo loop(total)", "  winner write-back", "CTA lifetime" };
     unsigned long long h[PR_N + 1];
     if (cudaMemcpy(h, e->d_prof, sizeof(h), cudaMemcpyDeviceToHost) == cudaSuccess) {
