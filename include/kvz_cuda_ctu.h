@@ -99,7 +99,7 @@ typedef struct kvz_cuda_ctu_device_result {
   const kvz_cuda_ctu_sao *sao;
   const void *rec;                  /* final picture: Y, U, V planes back to back, stride = width (/2) samples */
   int32_t cu_stride, width_in_lcu, height_in_lcu;
-  float search_kernel_ms;           /* device time of the picture's search launch(es), CUDA events on its stream */
+  float search_kernel_ms;           /* device time of the picture's search launch, from the device's global timer */
 } kvz_cuda_ctu_device_result;
 int kvz_cuda_ctu_submit_device(kvz_cuda_ctu_enc *enc, const uint8_t *d_y, const uint8_t *d_u, const uint8_t *d_v, int stride_y, int stride_c,
                                const uint8_t *ctx_init, double lambda, double lambda_sqrt, int qp);

@@ -26,7 +26,6 @@
 #include "strategyselector.h"
 #include "cu.h"
 #include "image.h"
-#include "rdo.h"
 #include "sao.h"
 #include "transform.h"
 
@@ -66,17 +65,9 @@ static void dequant_cuda(const encoder_state_t *const state, coeff_t *q_coef, co
   kvz_cuda_call_dequant(&p, q_coef, coef, width, type);
 }
 
-/* KVZ_CUDA_RDOQ_HOST=1 keeps kvz_rdoq on the host (forward half / host kvz_rdoq / inverse half), for A/B comparison */
-static int rdoq_on_host(void)
-{
-  static int v = -1;
-  if (v < 0) { const char *e = getenv("KVZ_CUDA_RDOQ_HOST"); v = (e && e[0] == '1') ? 1 : 0; }
-  return v;
-}
-
 /* ref: strategies-quant.h:51-57 (quant_residual_func), quant-generic.c:198-292.  With RDOQ, kvz_rdoq (not a strategy,
- * src/rdo.c:661) runs on the device too (csrc/rdoq.cuh); with KVZ_CUDA_RDOQ_HOST=1 the host's kvz_rdoq runs between
- * the device's forward and inverse halves, exactly where the generic and AVX2 versions call it. */
+ * src/rdo.c:661) runs on the device too (csrc/rdoq.cuh), between the forward and inverse halves, exactly where the
+ * generic and AVX2 versions call it. */
 static int quantize_residual_cuda(encoder_state_t *const state, const cu_info_t *const cur_cu, const int width,
                                   const color_t color, const coeff_scan_order_t scan_order, const int use_trskip,
                                   const int in_stride, const int out_stride, const kvz_pixel *const ref_in,
@@ -85,7 +76,7 @@ static int quantize_residual_cuda(encoder_state_t *const state, const cu_info_t 
   kvz_cuda_quant_params p; fill_qp(state, &p);
   const encoder_control_t *enc = state->encoder_control;
   const int intra = cur_cu->type == CU_INTRA;
-  if (enc->cfg.rdoq_enable && (width > 4 || !enc->cfg.rdoq_skip) && !rdoq_on_host()) {
+  if (enc->cfg.rdoq_enable && (width > 4 || !enc->cfg.rdoq_skip)) {
     /* kvz_rdoq on the device: the context models and lambda it reads are state->cabac.ctx and state->lambda (rdo.c:665-884) */
     _Static_assert(sizeof(kvz_cuda_cabac_ctx) == sizeof(((cabac_data_t *)0)->ctx), "cabac ctx image");
     kvz_cuda_rdoq_params rp = { state->lambda, state->qp, enc->bitdepth, enc->cfg.signhide_enable, 0 };
@@ -93,23 +84,6 @@ static int quantize_residual_cuda(encoder_state_t *const state, const cu_info_t 
     tr_depth += (cur_cu->part_size == SIZE_NxN ? 1 : 0);
     return kvz_cuda_call_quantize_residual_rdoq(&p, &rp, (const kvz_cuda_cabac_ctx *)&state->cabac.ctx, width, color, scan_order, use_trskip,
                                                 intra, early_skip, tr_depth, in_stride, out_stride, ref_in, pred_in, rec_out, coeff_out);
-  }
-  if (enc->cfg.rdoq_enable && (width > 4 || !enc->cfg.rdoq_skip)) {
-    ALIGNED(64) coeff_t coeff[TR_MAX_WIDTH * TR_MAX_WIDTH];
-    kvz_cuda_call_quantize_residual(&p, width, color, scan_order, use_trskip, intra, early_skip, 1, in_stride, out_stride,
-                                    ref_in, pred_in, rec_out, coeff);
-    int8_t tr_depth = cur_cu->tr_depth - cur_cu->depth;
-    tr_depth += (cur_cu->part_size == SIZE_NxN ? 1 : 0);
-    kvz_rdoq(state, coeff, coeff_out, width, width, (color == COLOR_Y ? 0 : 2), scan_order, cur_cu->type, tr_depth);
-    int has_coeffs = 0;
-    for (int i = 0; i < width * width; ++i) if (coeff_out[i] != 0) { has_coeffs = 1; break; }
-    if (has_coeffs && !early_skip) {
-      kvz_cuda_call_quantize_residual(&p, width, color, scan_order, use_trskip, intra, early_skip, 2, in_stride, out_stride,
-                                      ref_in, pred_in, rec_out, coeff_out);
-    } else if (rec_out != pred_in) {
-      for (int y = 0; y < width; ++y) memcpy(&rec_out[y * out_stride], &pred_in[y * in_stride], width * sizeof(kvz_pixel));
-    }
-    return has_coeffs;
   }
   return kvz_cuda_call_quantize_residual(&p, width, color, scan_order, use_trskip, intra, early_skip, 0, in_stride, out_stride,
                                          ref_in, pred_in, rec_out, coeff_out);

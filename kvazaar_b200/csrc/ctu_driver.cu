@@ -81,7 +81,7 @@ __global__ void __launch_bounds__(kThreads, 3) ctu_frame_kernel(const __grid_con
 {
   CtuST<Pix> *S = reinterpret_cast<CtuST<Pix> *>(ctu_smem_raw);
   __shared__ int s_ticket;
-  if (threadIdx.x == 0) S->leader_tid = a.sm_counter ? 32 * (atomicAdd(a.sm_counter + (sm_id() & 255), 1) & 3) : 0;
+  if (threadIdx.x == 0) S->leader_tid = 32 * (atomicAdd(a.sm_counter + (sm_id() & 255), 1) & 3);
   __syncthreads();
   CtxT<Pix> c = { a.T, &a.cfg, a.work + blockIdx.x, S };
 #if defined(KVZ_CTU_PROF)
@@ -133,23 +133,6 @@ __global__ void __launch_bounds__(kThreads, 3) ctu_frame_kernel(const __grid_con
   }
 }
 
-// Diagnostic alternative (KVZ_CUDA_CTU_DIAG=1): one launch per anti-diagonal, no inter-CTA waiting.
-template <typename Pix>
-__global__ void __launch_bounds__(kThreads, 3) ctu_diag_kernel(const __grid_constant__ KernelArgs<Pix> a, int diag, int cy_lo)
-{
-  CtuST<Pix> *S = reinterpret_cast<CtuST<Pix> *>(ctu_smem_raw);
-  if (threadIdx.x == 0) S->leader_tid = 0;
-  __syncthreads();
-  const int cy = cy_lo + blockIdx.x;
-  const int cx = diag - 2 * cy;
-  CtxT<Pix> c = { a.T, &a.cfg, a.work + blockIdx.x, S };
-#if defined(KVZ_CTU_PROF)
-  if (threadIdx.x == 0) for (int i = 0; i < PR_N; ++i) S->prof[i] = 0;
-  __syncthreads();
-#endif
-  ctu_job(c, &a.F, reinterpret_cast<SaoStats *>(S->arena), cx, cy);
-}
-
 template <typename Pix>
 __global__ void __launch_bounds__(kThreads) ctu_sao_apply_kernel(const __grid_constant__ KernelArgs<Pix> a)
 {
@@ -161,7 +144,6 @@ struct Slot {
   int state = 0;                 // 0 free, 1 submitted
   cudaStream_t stream = nullptr;
   cudaEvent_t done = nullptr;
-  cudaEvent_t k1 = nullptr;                 // after the search launches (diagnostic per-diagonal mode only)
   volatile unsigned long long *h_note = nullptr;   // pinned: written by the search launch's last CTA
   unsigned long long seq = 0;
   bool resident = false;
@@ -202,7 +184,7 @@ struct kvz_cuda_ctu_enc {
   int wl = 0, hl = 0, max_diag = 0, grid = 0;
   int pix = 1;                   // bytes per sample: 1 (8-bit) or 2 (10-bit)
   size_t plane_bytes = 0, smem = 0;
-  bool debug = false, diag_launches = false;
+  bool debug = false;
   std::vector<Slot> slots;
   std::mutex mtx;
   std::condition_variable cv;
@@ -242,7 +224,6 @@ void kvz_cuda_ctu_close(kvz_cuda_ctu_enc *e)
     cudaFreeHost(s.h_src); cudaFreeHost(s.h_out); cudaFreeHost(s.h_dbg); cudaFreeHost(s.h_cu); cudaFreeHost(s.h_coeff); cudaFreeHost(s.h_sao);
     cudaFreeHost(s.h_row_ctx); cudaFreeHost(s.h_dbg_ctx);
     if (s.done) cudaEventDestroy(s.done);
-    if (s.k1) cudaEventDestroy(s.k1);
     cudaFreeHost((void *)s.h_note);
     if (s.stream) cudaStreamDestroy(s.stream);
   }
@@ -272,7 +253,7 @@ template <typename Pix> static void init_args(kvz_cuda_ctu_enc *e, Slot &s, Kern
   const int W = e->cfg.width, H = e->cfg.height;
   a.T = e->d_tables;
   a.work = (CtuWorkT<Pix> *)s.d_work; a.sao_stats = s.d_stats; a.dbg_ctx = s.d_dbg_ctx;
-  a.order = e->d_order; a.sync = s.d_sync; a.nctu = e->wl * e->hl; a.prof = e->d_prof; a.sm_counter = getenv("KVZ_CUDA_CTU_LEADER0") ? nullptr : e->d_sm_counter;   // (A/B switch: leader always warp 0)
+  a.order = e->d_order; a.sync = s.d_sync; a.nctu = e->wl * e->hl; a.prof = e->d_prof; a.sm_counter = e->d_sm_counter;
   FrameDevT<Pix> &F = a.F;
   const size_t ysz = (size_t)W * H, csz = ysz / 4, plane = ysz + 2 * csz;
   Pix *p = (Pix *)s.d_planes;
@@ -306,12 +287,10 @@ kvz_cuda_ctu_enc *kvz_cuda_ctu_open(const kvz_cuda_ctu_config *cfg, int slots)
     if (hi - lo + 1 > e->max_diag) e->max_diag = hi - lo + 1;
     for (int cy = lo; cy <= hi; ++cy) { order.push_back((uint16_t)(d - 2 * cy)); order.push_back((uint16_t)cy); }
   }
-  e->diag_launches = getenv("KVZ_CUDA_CTU_DIAG") != nullptr;
   // persistent CTAs per picture: 40 % of the widest diagonal (the average wavefront is about half of it; a smaller grid
-  // leaves fewer CTAs waiting idle and lets more pictures be resident at once); KVZ_CUDA_CTU_GRID overrides
-  e->grid = e->diag_launches ? e->max_diag : (e->max_diag * 2 + 4) / 5;
+  // leaves fewer CTAs waiting idle and lets more pictures be resident at once)
+  e->grid = (e->max_diag * 2 + 4) / 5;
   if (e->grid < 1) e->grid = 1;
-  if (const char *g = getenv("KVZ_CUDA_CTU_GRID")) { const int v = atoi(g); if (v > 0 && !e->diag_launches) e->grid = v < e->max_diag ? v : e->max_diag; }
   e->pix = cfg->bitdepth == 10 ? 2 : 1;
   e->plane_bytes = (size_t)W * H * 3 / 2 * e->pix;
   e->smem = e->pix == 2 ? sizeof(CtuST<uint16_t>) : sizeof(CtuST<uint8_t>);
@@ -332,13 +311,8 @@ kvz_cuda_ctu_enc *kvz_cuda_ctu_open(const kvz_cuda_ctu_config *cfg, int slots)
   CTU_CHECK_PTR(cudaMemset(e->d_sm_counter, 0, 256 * sizeof(int)));
   CTU_CHECK_PTR(cudaMalloc(&e->d_order, order.size() * sizeof(uint16_t)));
   CTU_CHECK_PTR(cudaMemcpy(e->d_order, order.data(), order.size() * sizeof(uint16_t), cudaMemcpyHostToDevice));
-  if (e->pix == 2) {
-    CTU_CHECK_PTR(cudaFuncSetAttribute(ctu_frame_kernel<uint16_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)e->smem));
-    CTU_CHECK_PTR(cudaFuncSetAttribute(ctu_diag_kernel<uint16_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)e->smem));
-  } else {
-    CTU_CHECK_PTR(cudaFuncSetAttribute(ctu_frame_kernel<uint8_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)e->smem));
-    CTU_CHECK_PTR(cudaFuncSetAttribute(ctu_diag_kernel<uint8_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)e->smem));
-  }
+  if (e->pix == 2) CTU_CHECK_PTR(cudaFuncSetAttribute(ctu_frame_kernel<uint16_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)e->smem));
+  else CTU_CHECK_PTR(cudaFuncSetAttribute(ctu_frame_kernel<uint8_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)e->smem));
   e->slots.resize(slots > 0 ? (slots > 512 ? 512 : slots) : 1);
   const size_t nctu = (size_t)e->wl * e->hl;
   const size_t cu_n = (size_t)(e->wl * 16) * (e->hl * 16);
@@ -346,7 +320,6 @@ kvz_cuda_ctu_enc *kvz_cuda_ctu_open(const kvz_cuda_ctu_config *cfg, int slots)
   for (Slot &s : e->slots) {
     CTU_CHECK_PTR(cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking));
     CTU_CHECK_PTR(cudaEventCreateWithFlags(&s.done, cudaEventDisableTiming));
-    CTU_CHECK_PTR(cudaEventCreateWithFlags(&s.k1, cudaEventDisableTiming));
     CTU_CHECK_PTR(cudaHostAlloc((void **)&s.h_note, 64, cudaHostAllocDefault));
     memset((void *)s.h_note, 0, 64);
     CTU_CHECK_PTR(cudaMalloc(&s.d_planes, e->plane_bytes * 4));
@@ -379,28 +352,17 @@ kvz_cuda_ctu_enc *kvz_cuda_ctu_open(const kvz_cuda_ctu_config *cfg, int slots)
 
 }  // extern "C"
 
-// the search launch(es) of a submitted picture
+// the search launch of a submitted picture
 template <typename Pix> static int launch_search(kvz_cuda_ctu_enc *e, Slot &s, double lambda, double lambda_sqrt, int qp)
 {
   KernelArgs<Pix> &a = args_of<Pix>(s);
-  cudaStream_t st = s.stream;
   a.cfg = e->cfg;
   a.cfg.lambda = lambda; a.cfg.lambda_sqrt = lambda_sqrt; a.cfg.qp = qp;
   a.host_note = s.h_note;
   a.seq = s.seq;
-  if (e->diag_launches) {
-    for (int d = 0; d < e->wl + 2 * (e->hl - 1); ++d) {
-      const int lo = d - (e->wl - 1) > 0 ? (d - (e->wl - 1) + 1) / 2 : 0, hi = d / 2 < e->hl - 1 ? d / 2 : e->hl - 1;
-      if (hi < lo) continue;
-      ctu_diag_kernel<Pix><<<hi - lo + 1, kThreads, e->smem, st>>>(a, d, lo);
-      e->launches.fetch_add(1, std::memory_order_relaxed);
-      kvzc::g_launches.fetch_add(1, std::memory_order_relaxed);
-    }
-  } else {
-    ctu_frame_kernel<Pix><<<e->grid, kThreads, e->smem, st>>>(a);
-    e->launches.fetch_add(1, std::memory_order_relaxed);
-    kvzc::g_launches.fetch_add(1, std::memory_order_relaxed);
-  }
+  ctu_frame_kernel<Pix><<<e->grid, kThreads, e->smem, s.stream>>>(a);
+  e->launches.fetch_add(1, std::memory_order_relaxed);
+  kvzc::g_launches.fetch_add(1, std::memory_order_relaxed);
   return 0;
 }
 
@@ -445,7 +407,6 @@ static int submit_picture(kvz_cuda_ctu_enc *e, const void *y, const void *u, con
   s.seq += 1;
   if (e->pix == 2) launch_search<uint16_t>(e, s, lambda, lambda_sqrt, qp);
   else launch_search<uint8_t>(e, s, lambda, lambda_sqrt, qp);
-  if (e->diag_launches) KVZC_CHECK(cudaEventRecord(s.k1, st));
   KVZC_CHECK(cudaGetLastError());
   s.resident = resident;
   return id;
@@ -457,14 +418,11 @@ static int submit_picture(kvz_cuda_ctu_enc *e, const void *y, const void *u, con
 // block the pictures of other streams queued behind it -- only one picture per queue would run.
 static int finish_picture(kvz_cuda_ctu_enc *e, Slot &s)
 {
-  if (e->diag_launches) KVZC_CHECK(cudaEventSynchronize(s.k1));
-  else {
-    // sleep-poll the completion note (the host threads are needed by the encoder's CABAC stage)
-    unsigned spins = 0;
-    while (__atomic_load_n((const unsigned long long *)s.h_note, __ATOMIC_ACQUIRE) != s.seq) {
-      if (++spins > 20) { struct timespec ts = { 0, 200000 }; nanosleep(&ts, nullptr); }
-      if ((spins & 1023) == 0) { const cudaError_t err = cudaStreamQuery(s.stream); if (err != cudaSuccess && err != cudaErrorNotReady) KVZC_CHECK(err); }
-    }
+  // sleep-poll the completion note (the host threads are needed by the encoder's CABAC stage)
+  unsigned spins = 0;
+  while (__atomic_load_n((const unsigned long long *)s.h_note, __ATOMIC_ACQUIRE) != s.seq) {
+    if (++spins > 20) { struct timespec ts = { 0, 200000 }; nanosleep(&ts, nullptr); }
+    if ((spins & 1023) == 0) { const cudaError_t err = cudaStreamQuery(s.stream); if (err != cudaSuccess && err != cudaErrorNotReady) KVZC_CHECK(err); }
   }
   cudaStream_t st = s.stream;
   if (e->pix == 2) ctu_sao_apply_kernel<uint16_t><<<e->wl * e->hl, kThreads, 0, st>>>(s.args16);
@@ -512,7 +470,7 @@ int kvz_cuda_ctu_wait_device(kvz_cuda_ctu_enc *e, int slot, kvz_cuda_ctu_device_
   out->rec = s.d_planes + 2 * e->plane_bytes;
   out->cu_stride = e->wl * 16;
   out->width_in_lcu = e->wl; out->height_in_lcu = e->hl;
-  if (!e->diag_launches) out->search_kernel_ms = (float)((double)(s.h_note[2] - s.h_note[1]) * 1e-6);   // globaltimer ns of first / last CTA
+  out->search_kernel_ms = (float)((double)(s.h_note[2] - s.h_note[1]) * 1e-6);   // globaltimer ns of first / last CTA
   return 0;
 }
 

@@ -510,18 +510,6 @@ static int launch_recon_phase(const kvz_cuda_quant_params &qp, const T *src, con
   return 0;
 }
 
-// first minimum of the 35 mode costs of every block (the 16-bit rough search writes full cost tables)
-__global__ void __launch_bounds__(256) rough_argmin_kernel(const uint32_t *__restrict__ costs, int nblk, int8_t *__restrict__ best_mode,
-                                                           uint32_t *__restrict__ best_cost)
-{
-  const int b = blockIdx.x * blockDim.x + threadIdx.x;
-  if (b >= nblk) return;
-  uint32_t bc = costs[(size_t)b * 35];
-  int bm = 0;
-  for (int m = 1; m < 35; ++m) { const uint32_t c = costs[(size_t)b * 35 + m]; if (c < bc) { bc = c; bm = m; } }
-  best_mode[b] = (int8_t)bm; best_cost[b] = bc;
-}
-
 // 4x4 luma with transform skip (PHASE 0 fused / 1 forward / 2 inverse)
 template <int PHASE, class T>
 static int launch_recon_trskip(const kvz_cuda_quant_params &qp, const T *src, const T *rin, int stride, int pic_w, int pic_h,
@@ -584,7 +572,7 @@ struct kvz_cuda_frame_pass {
   size_t host_bytes, total_bytes;
   uint8_t *blob = nullptr;              // device: host-visible sections first, device-only sections after
   // device-only
-  size_t off_rec_y[4], off_rec_u[3], off_rec_v[3], off_costs35[4] = {};
+  size_t off_rec_y[4], off_rec_u[3], off_rec_v[3];
   size_t off_sao_off, off_dbk_cus, off_cabac, off_src_copy, off_compact, off_tile_counts;
   size_t off_ts_rec = 0, off_ts_coeff = 0, off_ts_has = 0, off_ts_ssd = 0, off_ts_bits = 0;
   kvz_cuda_rdoq_params rdoq;
@@ -593,7 +581,6 @@ struct kvz_cuda_frame_pass {
   // optional per-stage CUDA-event timing (bench.py's live roofline measurement)
   bool timing = false;
   cudaEvent_t ev[KVZ_CUDA_FP_STAGES + 1] = {};
-  bool rough_v1 = getenv("KVZ_CUDA_ROUGH_V1") != nullptr;   // A/B switch of the 16-bit rough search, read once
   double ms_acc[KVZ_CUDA_FP_STAGES] = {};
   int runs_timed = 0;
   bool ev_pending = false;
@@ -670,7 +657,6 @@ static kvz_cuda_frame_pass *fp_build(const kvz_cuda_fp_params *p, bool alloc)
   fp->off_tile_counts = take(4 * ((size_t)L.n_chunks / 1024 + 2));
   for (int d = 0; d < 4; ++d) fp->off_rec_y[d] = take((size_t)W * H * px);
   for (int d = 0; d < 3; ++d) { fp->off_rec_u[d] = take((size_t)W * H / 4 * px); fp->off_rec_v[d] = take((size_t)W * H / 4 * px); }
-  if (px == 2) for (int d = 0; d < 4; ++d) fp->off_costs35[d] = take(4 * (size_t)fp->nblk[d] * 35);   // 16-bit rough search writes cost tables
   fp->off_sao_off = take(4 * (size_t)4 * fp->nctu3 * 5);
   fp->off_src_copy = take((size_t)W * H * 3 / 2 * px);
   // deblocking input: the CU records of the uniform 8x8 intra quadtree whose reconstruction SAO works on
@@ -746,15 +732,9 @@ static int fp_run_dev_t(kvz_cuda_frame_pass *fp, const void *src_dev, const void
     fp_mark(fp, s0 + 0, st);
     if (nb == 0) { for (int k = 1; k < 9; ++k) fp_mark(fp, s0 + k, st); continue; }
     int8_t *modes = (int8_t *)(B + L.mode_y[d]);
+    // rough search with the mode selection fused in; the 35-entry cost tables stay on chip
     if constexpr (BD == 8) {
-      // rough search with the mode selection fused in; the 35-entry cost tables stay on chip
       if (int r = rough_search_u8(log2w, src, rin, W, W, H, nullptr, modes, (uint32_t *)(B + L.cost_y[d]), st)) return r;
-    } else if (fp->rough_v1) {
-      // A/B switch: the straightforward per-pixel rough-search kernel (intra.cu) + argmin
-      uint32_t *costs = (uint32_t *)(B + fp->off_costs35[d]);
-      if (int r = kvz_cuda_intra_rough_search_frame(log2w, BD, src, rin, W, W, H, costs, st)) return r;
-      rough_argmin_kernel<<<(nb + 255) / 256, 256, 0, st>>>(costs, nb, modes, (uint32_t *)(B + L.cost_y[d]));
-      KVZC_LAUNCHED();
     } else {
       if (int r = rough_search_u16(log2w, src, rin, W, W, H, nullptr, modes, (uint32_t *)(B + L.cost_y[d]), st)) return r;
     }

@@ -1,9 +1,7 @@
-// intra.cu -- intra group: batched prediction, reference building and the fused frame-level rough search.
-#include <stdlib.h>
-
+// intra.cu -- intra group: batched prediction, reference building and the entry point of the fused frame-level rough
+// search (rough_search.cu).
 #include "common.cuh"
 #include "intra.cuh"
-#include "satd.cuh"
 
 namespace kvzc {
 
@@ -64,106 +62,6 @@ __global__ void __launch_bounds__(128) build_reference_kernel(int log2w, int col
   }
 }
 
-// ---------------------------------------------------------------------------------------------
-// Fused frame-level rough search.  One CTA per w x w block of the luma plane:
-//   refs (built from rec_plane) -> smoothed refs -> for every (mode, 8x8 sub-block): the thread predicts its 64
-//   samples straight into registers and runs the packed 8x8 Hadamard against the source -> per-mode sums.
-// Nothing but the source/reconstruction tile is read and nothing but 35 costs is written: predictions never
-// exist in memory.  (search_intra_rough's inner loop, ref: search_intra.c:391-530, for all 35 modes.)
-// ---------------------------------------------------------------------------------------------
-template <class T, int LOG2W>
-__global__ void __launch_bounds__(LOG2W == 2 ? 64 : 128) rough_search_kernel(const T *__restrict__ src, const T *__restrict__ rec,
-                                                                             int stride, int pic_w, int pic_h, int blocks_x,
-                                                                             uint32_t *__restrict__ costs)
-{
-  constexpr int W = 1 << LOG2W, N = 2 * W + 1;
-  constexpr int S = W >= 8 ? W / 8 : 1, SUBS = S * S;
-  constexpr int SHIFT = PixTraits<T>::kBits - 8;
-  __shared__ T s_top[N + 3], s_left[N + 3], s_ftop[N + 3], s_fleft[N + 3];
-  __shared__ __align__(16) T s_src[W * W];
-  __shared__ uint32_t s_cost[35];
-  __shared__ int s_dc;
-  const int bx = blockIdx.x % blocks_x, by = blockIdx.x / blocks_x;
-  const int x0 = bx * W, y0 = by * W;
-  const BuildRefCtx c = build_ref_ctx(LOG2W, 0, x0, y0, pic_w, pic_h);
-  for (int i = threadIdx.x; i < 2 * N; i += blockDim.x) {
-    const bool is_top = i < N;
-    const int k = is_top ? i : i - N;
-    (is_top ? s_top : s_left)[k] = (T)build_ref_entry(c, rec, stride, is_top, k);
-  }
-  for (int i = threadIdx.x; i < W * W; i += blockDim.x) s_src[i] = src[(long)(y0 + i / W) * stride + x0 + (i % W)];
-  if (threadIdx.x < 35) s_cost[threadIdx.x] = 0;
-  __syncthreads();
-  for (int i = threadIdx.x; i < 2 * N; i += blockDim.x) {
-    const bool is_top = i < N;
-    const int k = is_top ? i : i - N;
-    (is_top ? s_ftop : s_fleft)[k] = (T)filter_ref_entry(s_top, s_left, is_top, k, N);
-  }
-  if (threadIdx.x == 0) s_dc = dc_value(LOG2W, s_top, s_left);
-  __syncthreads();
-  const int dc = s_dc;
-  for (int item = threadIdx.x; item < 35 * SUBS; item += blockDim.x) {
-    const int mode = item / SUBS, sub = item - mode * SUBS;
-    const int sy = (sub / S) * 8, sx = (sub % S) * 8;
-    uint32_t cost;
-    if constexpr (W == 4) {
-      if constexpr (sizeof(T) == 1) {
-        uint32_t ra[4], rb[4];
-#pragma unroll
-        for (int y = 0; y < 4; ++y) {
-          uint32_t p = 0;
-#pragma unroll
-          for (int x = 0; x < 4; ++x)
-            p |= (uint32_t)intra_predict_px(LOG2W, mode, 0, true, s_top, s_left, s_ftop, s_fleft, dc, x, y) << (8 * x);
-          rb[y] = p;
-          ra[y] = *reinterpret_cast<const uint32_t *>(&s_src[y * 4]);
-        }
-        cost = (hadamard4x4_u8(ra, rb) + 1) >> 1;
-      } else {
-        int d[4][4];
-#pragma unroll
-        for (int y = 0; y < 4; ++y)
-#pragma unroll
-          for (int x = 0; x < 4; ++x)
-            d[y][x] = (int)s_src[y * 4 + x] - intra_predict_px(LOG2W, mode, 0, true, s_top, s_left, s_ftop, s_fleft, dc, x, y);
-        cost = (hadamard_abs_sum_i32<4>(d) + 1) >> 1;
-      }
-      costs[(size_t)blockIdx.x * 35 + mode] = cost;          // satd_4x4 has no bit-depth shift
-    } else {
-      if constexpr (sizeof(T) == 1) {
-        uint2 ra[8], rb[8];
-#pragma unroll
-        for (int y = 0; y < 8; ++y) {
-          uint32_t lo = 0, hi = 0;
-#pragma unroll
-          for (int x = 0; x < 4; ++x) {
-            lo |= (uint32_t)intra_predict_px(LOG2W, mode, 0, true, s_top, s_left, s_ftop, s_fleft, dc, sx + x, sy + y) << (8 * x);
-            hi |= (uint32_t)intra_predict_px(LOG2W, mode, 0, true, s_top, s_left, s_ftop, s_fleft, dc, sx + 4 + x, sy + y) << (8 * x);
-          }
-          rb[y] = make_uint2(lo, hi);
-          ra[y] = *reinterpret_cast<const uint2 *>(&s_src[(sy + y) * W + sx]);
-        }
-        cost = (hadamard8x8_u8(ra, rb) + 2) >> 2;
-      } else {
-        int d[8][8];
-#pragma unroll
-        for (int y = 0; y < 8; ++y)
-#pragma unroll
-          for (int x = 0; x < 8; ++x)
-            d[y][x] = (int)s_src[(sy + y) * W + sx + x] -
-                      intra_predict_px(LOG2W, mode, 0, true, s_top, s_left, s_ftop, s_fleft, dc, sx + x, sy + y);
-        cost = (hadamard_abs_sum_i32<8>(d) + 2) >> 2;
-      }
-      if (SUBS == 1) costs[(size_t)blockIdx.x * 35 + mode] = cost >> SHIFT;
-      else atomicAdd(&s_cost[mode], cost);
-    }
-  }
-  if (SUBS > 1) {
-    __syncthreads();
-    if (threadIdx.x < 35) costs[(size_t)blockIdx.x * 35 + threadIdx.x] = s_cost[threadIdx.x] >> SHIFT;
-  }
-}
-
 }  // namespace kvzc
 
 using namespace kvzc;
@@ -173,22 +71,6 @@ int rough_search_u8(int log2w, const uint8_t *src, const uint8_t *rec, int strid
                     int8_t *best_mode, uint32_t *best_cost, cudaStream_t st);
 int rough_search_u16(int log2w, const uint16_t *src, const uint16_t *rec, int stride, int pic_w, int pic_h, uint32_t *costs,
                      int8_t *best_mode, uint32_t *best_cost, cudaStream_t st);
-}
-
-template <class T>
-static int launch_rough(int log2w, const T *src, const T *rec, int stride, int pic_w, int pic_h, uint32_t *costs, cudaStream_t st)
-{
-  const int w = 1 << log2w;
-  const int bx = pic_w / w, by = pic_h / w;
-  if (bx * by == 0) return 0;
-  switch (log2w) {
-    case 2: rough_search_kernel<T, 2><<<bx * by, 64, 0, st>>>(src, rec, stride, pic_w, pic_h, bx, costs); break;
-    case 3: rough_search_kernel<T, 3><<<bx * by, 128, 0, st>>>(src, rec, stride, pic_w, pic_h, bx, costs); break;
-    case 4: rough_search_kernel<T, 4><<<bx * by, 128, 0, st>>>(src, rec, stride, pic_w, pic_h, bx, costs); break;
-    default: rough_search_kernel<T, 5><<<bx * by, 128, 0, st>>>(src, rec, stride, pic_w, pic_h, bx, costs); break;
-  }
-  KVZC_LAUNCHED();
-  return 0;
 }
 
 extern "C" {
@@ -232,15 +114,9 @@ int kvz_cuda_intra_rough_search_frame(int log2_width, int bitdepth, const void *
 {
   KVZC_REQUIRE_DEVICE();
   KVZC_ARG(src_plane && rec_plane && costs && log2_width >= 2 && log2_width <= 5 && pic_w % 8 == 0 && pic_h % 8 == 0);
-  // tuned kernel (rough_search.cu); KVZ_CUDA_ROUGH_V1=1 selects the straightforward one for A/B checks
-  static const bool v1 = getenv("KVZ_CUDA_ROUGH_V1") != nullptr;
-  if (bitdepth != 8 && !v1)
-    return rough_search_u16(log2_width, (const uint16_t *)src_plane, (const uint16_t *)rec_plane, stride, pic_w, pic_h, costs, nullptr, nullptr, as_stream(stream));
-  if (bitdepth == 8) {
-    if (!v1) return rough_search_u8(log2_width, (const uint8_t *)src_plane, (const uint8_t *)rec_plane, stride, pic_w, pic_h, costs, nullptr, nullptr, as_stream(stream));
-    return launch_rough<uint8_t>(log2_width, (const uint8_t *)src_plane, (const uint8_t *)rec_plane, stride, pic_w, pic_h, costs, as_stream(stream));
-  }
-  return launch_rough<uint16_t>(log2_width, (const uint16_t *)src_plane, (const uint16_t *)rec_plane, stride, pic_w, pic_h, costs, as_stream(stream));
+  if (bitdepth == 8)
+    return rough_search_u8(log2_width, (const uint8_t *)src_plane, (const uint8_t *)rec_plane, stride, pic_w, pic_h, costs, nullptr, nullptr, as_stream(stream));
+  return rough_search_u16(log2_width, (const uint16_t *)src_plane, (const uint16_t *)rec_plane, stride, pic_w, pic_h, costs, nullptr, nullptr, as_stream(stream));
 }
 
 }  // extern "C"

@@ -1,7 +1,5 @@
 // picture.cu -- picture-group kernels: SAD / SATD / SSD families, bipred average, pixel variance.
 // Reference behaviour: src/strategies/generic/picture-generic.c, strategies-picture.h:53-113.
-#include <stdlib.h>
-
 #include "common.cuh"
 #include "satd.cuh"
 
@@ -292,10 +290,6 @@ __global__ void pixel_var_kernel(const T *__restrict__ buf, uint32_t len, int co
 
 using namespace kvzc;
 
-namespace kvzc {
-int satd8_tma(const uint8_t *a, const uint8_t *b, int count, uint32_t *out, cudaStream_t st);
-}
-
 extern "C" {
 
 int kvz_cuda_sad_nxn_batch(int n, int bitdepth, const void *a, const void *b, int count, uint32_t *out, void *stream)
@@ -310,12 +304,6 @@ int kvz_cuda_satd_nxn_batch(int n, int bitdepth, const void *a, const void *b, i
 {
   KVZC_REQUIRE_DEVICE();
   KVZC_ARG(a && b && out && count >= 0);
-  if (bitdepth == 8 && n == 8 && count >= 4096 && (((uintptr_t)a | (uintptr_t)b) & 15) == 0) {
-    // KVZ_CUDA_SATD_TMA=1 selects the persistent TMA-fed variant (satd_tma.cu).  The plain 128-bit-load kernel keeps
-    // 3x more warps in flight for this issue-bound arithmetic, so it stays the default (tools/time_satd.py times both).
-    static const bool tma = getenv("KVZ_CUDA_SATD_TMA") != nullptr;
-    if (tma) return satd8_tma((const uint8_t *)a, (const uint8_t *)b, count, out, as_stream(stream));
-  }
   if (bitdepth == 8) return launch_nxn<uint8_t, true>(n, (const uint8_t *)a, (const uint8_t *)b, n * n, 0, 1, count, out, as_stream(stream));
   return launch_nxn<uint16_t, true>(n, (const uint16_t *)a, (const uint16_t *)b, n * n, 0, 1, count, out, as_stream(stream));
 }

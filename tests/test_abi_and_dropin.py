@@ -91,7 +91,7 @@ def test_reference_greatest_suites_over_cuda_entries():
 DROPIN_CASES = [
     # BASELINE.json configs[0]: 64x64 ultrafast -q 32 -p 1
     ("cfg0_ultrafast_intra", 64, 64, 2, ["preset=ultrafast", "qp=32", "period=1"]),
-    # medium (RDOQ through the host's kvz_rdoq between our forward and inverse halves, SAO full)
+    # medium (RDOQ on the device between our forward and inverse halves, SAO full)
     ("medium_intra_rdoq_sao", 64, 64, 1, ["preset=medium", "qp=27", "period=1"]),
     # inter: hexbs ME, fractional ME (FME filters), bipred, merge -> ipol + sad + satd_any_size(+quad)
     ("fast_inter", 128, 64, 3, ["preset=fast", "qp=30", "period=16", "gop=0"]),

@@ -34,11 +34,8 @@ def test_sad_satd_nxn_batch(cuda_lib, orc, n):
         assert satd[i] == orc.satd_nxn(n, ai, bi), (n, i)
 
 
-def test_satd8_tma_path_large_batch(cuda_lib, orc, monkeypatch):
-    """KVZ_CUDA_SATD_TMA=1 + count >= 4096 takes the persistent TMA-fed kernel (satd_tma.cu); the odd count exercises
-    the partial last tile.  (The flag is read once per process: set it before the first large batch.)"""
-    import os
-    os.environ["KVZ_CUDA_SATD_TMA"] = "1"
+def test_satd8_large_batch(cuda_lib, orc):
+    """A batch of more than 4096 pairs; the odd count exercises a partial last CTA."""
     kb = cuda_lib
     r = cs.rng(1050)
     count = 3 * 4096 + 77
@@ -48,7 +45,7 @@ def test_satd8_tma_path_large_batch(cuda_lib, orc, monkeypatch):
     got = host(kb.satd_nxn_batch(8, dev(kb, a), dev(kb, b), count))
     for i in list(range(0, 600)) + list(range(count - 300, count)) + list(range(4000, 4200)):
         assert got[i] == orc.satd_nxn(8, cs.al(a[i * 64:(i + 1) * 64]), cs.al(b[i * 64:(i + 1) * 64])), i
-    # and the whole batch against the plain kernel (multi entry point with one mode never takes the TMA path)
+    # and the whole batch against the multi-mode entry point with one mode
     plain = host(kb.cost_nxn_multi_batch(1, 8, dev(kb, a), 64, 0, 1, dev(kb, b), count)).ravel()
     assert np.array_equal(got, plain)
 

@@ -1,6 +1,5 @@
 """Times kvz_cuda_satd_nxn_batch(8) -- the HBM-streaming kernel of the north star -- on 4 Mi block pairs (512 MiB of input,
-more than L2) with CUDA events; KVZ_CUDA_SATD_TMA=1 picks the TMA variant.  `--json`: one JSON object (bench.py attaches it
-to its line as "roofline_satd_batch")."""
+more than L2) with CUDA events.  `--json`: one JSON object (bench.py attaches it to its line as "roofline_satd_batch")."""
 import json
 import os
 import sys
@@ -28,9 +27,9 @@ if os.path.exists(mp):
     peak, src = float(json.load(open(mp))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
 alg = n * 132                      # SURVEY 8(d): 2 * 64 bytes in + 4 bytes out per 8x8 pair
 if "--json" in sys.argv:
-    print(json.dumps({"kernel": "satd_nxn_kernel<u8,8> (kvz_cuda_satd_nxn_batch)" if not os.environ.get("KVZ_CUDA_SATD_TMA") else "satd8_tma_kernel",
+    print(json.dumps({"kernel": "satd_nxn_kernel<u8,8> (kvz_cuda_satd_nxn_batch)",
                       "bound": "hbm", "achieved": alg / ms / 1e6, "peak": peak, "unit": "GB/s", "frac": alg / ms / 1e6 / peak, "traffic": None,
                       "ms_per_launch": ms, "pairs_per_launch": n, "algorithmic_bytes_per_launch": alg, "peak_source": src,
                       "checksum": int(o.to(torch.int64).sum()), "timing": "CUDA events over 20 launches after 3 warm-up launches; inputs (512 MiB) exceed L2"}))
 else:
-    print("tma" if os.environ.get("KVZ_CUDA_SATD_TMA") else "plain", f"{ms:.4f} ms  {alg / ms / 1e6:.0f} GB/s  frac {alg / ms / 1e6 / peak:.3f}  sum {int(o.to(torch.int64).sum())}")
+    print(f"{ms:.4f} ms  {alg / ms / 1e6:.0f} GB/s  frac {alg / ms / 1e6 / peak:.3f}  sum {int(o.to(torch.int64).sum())}")
