@@ -9,8 +9,8 @@ SRCS      := $(wildcard $(SRCDIR)/*.cu)
 OBJS      := $(patsubst $(SRCDIR)/%.cu,$(OBJDIR)/%.o,$(SRCS))
 LIB       := kvazaar_b200/libkvzcuda.so
 
-.PHONY: all lib oracle ref clean
-all: lib oracle ref
+.PHONY: all lib probe oracle ref clean
+all: lib probe oracle ref
 lib: $(LIB)
 
 # make PROF=1: the CTU driver with its phase profile (diagnostic; kvz_cuda_ctu_close prints it)
@@ -31,10 +31,21 @@ $(OBJDIR)/%.o: $(SRCDIR)/%.cu $(wildcard $(SRCDIR)/*.cuh) include/kvz_cuda.h
 $(LIB): $(OBJS)
 	$(NVCC) $(ARCH) -shared -o $@ $(OBJS) -lcudart -ldl -lpthread
 
+# test infrastructure: the CTU search driver's transform-unit jobs behind a C entry point (tests/test_ctu_tu_jobs.py),
+# built with the product's flags (sm_90a) and for the host with the one-thread CTA (g++), which the device's results are
+# compared with; never linked into the product library
+PROBE     := tests/cuda/libkvzctu_probe.so
+PROBE_HOST := tests/hostsim/libkvzctu_probe_host.so
+probe: $(PROBE) $(PROBE_HOST)
+$(PROBE): tests/cuda/ctu_tu_probe.cu $(wildcard $(SRCDIR)/ctu/*.h)
+	$(NVCC) $(ARCH) -O3 -std=c++17 -fmad=false -Xcompiler -fPIC,-Wall -shared -o $@ $< -lcudart
+$(PROBE_HOST): tests/cuda/ctu_tu_probe.cu $(wildcard $(SRCDIR)/ctu/*.h)
+	g++ -O2 -g -std=c++17 -fPIC -shared -ffp-contract=off -Wall -Wno-unused-function -Wno-unknown-pragmas -x c++ -o $@ $<
+
 oracle:
 	$(MAKE) -s -C oracle oracle
 ref:
 	$(MAKE) -s -C oracle ref
 
 clean:
-	rm -rf build $(LIB)
+	rm -rf build $(LIB) $(PROBE) $(PROBE_HOST)

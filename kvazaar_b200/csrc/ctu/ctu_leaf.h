@@ -188,6 +188,36 @@ template <typename Pix> CTU_FN Plane<Pix> plane_of(CtuWorkT<Pix> *W, LcuLevel<Pi
 }
 
 // ------------------------------------------------------------------------------------------------ intra references
+// The [1 2 1] smoothing of the luma references and the DC sum of every colour in `mask`, from the unfiltered references
+// r[colour].top / .left of blocks of log2w[colour] (the tail of build_refs_multi).  n0: the number of luma references
+// per edge, 2 * (1 << log2w[0]) + 1, or 0 when `mask` has no luma.
+template <typename Pix> CTU_FN void refs_smooth_dc(const int log2w[3], int mask, int n0, IntraRefs<Pix> *r)
+{
+  // smoothing of the luma references; one thread per colour sums the DC
+  #pragma unroll 1
+  for (int i = CTU_TID; i < 2 * n0 + 3; i += CTU_NT) {
+    if (i >= 2 * n0) {
+      const int color = i - 2 * n0;
+      if ((mask >> color) & 1) {
+        const int w = 1 << log2w[color];
+        int s = 0;
+        for (int k = 1; k <= w; ++k) s += r[color].top[k] + r[color].left[k];
+        r[color].dc = (s + w) >> (log2w[color] + 1);
+      }
+      continue;
+    }
+    const bool is_top = i >= n0;
+    const int e = is_top ? i - n0 : i;
+    const Pix *p = is_top ? r[0].top : r[0].left;
+    int v;
+    if (e == 0) v = (r[0].left[1] + 2 * r[0].left[0] + r[0].top[1] + 2) >> 2;
+    else if (e == n0 - 1) v = p[e];
+    else v = (p[e - 1] + 2 * p[e] + p[e + 1] + 2) >> 2;
+    (is_top ? r[0].ftop : r[0].fleft)[e] = (Pix)v;
+  }
+  CTU_SYNC();
+}
+
 // kvz_intra_build_reference for the blocks of the colours in `mask` (bit per colour) at luma position (x, y) (picture
 // coordinates), into r[colour], followed by the [1 2 1] smoothing (done eagerly: the reference's lazy flag only saves
 // time; chroma never reads it) and the DC sum.  log2w[colour]: the block sizes.  One pass over all colours: the border
@@ -234,30 +264,7 @@ template <typename Pix> CTU_FN_NOINLINE void build_refs_multi(const SmTables *T,
     (is_top ? r[color].top : r[color].left)[e] = (Pix)v;
   }
   CTU_SYNC();
-  // smoothing of the luma references; one thread per colour sums the DC
-  const int n0 = n_of[0];
-  #pragma unroll 1
-  for (int i = CTU_TID; i < 2 * n0 + 3; i += CTU_NT) {
-    if (i >= 2 * n0) {
-      const int color = i - 2 * n0;
-      if ((mask >> color) & 1) {
-        const int w = 1 << log2w[color];
-        int s = 0;
-        for (int k = 1; k <= w; ++k) s += r[color].top[k] + r[color].left[k];
-        r[color].dc = (s + w) >> (log2w[color] + 1);
-      }
-      continue;
-    }
-    const bool is_top = i >= n0;
-    const int e = is_top ? i - n0 : i;
-    const Pix *p = is_top ? r[0].top : r[0].left;
-    int v;
-    if (e == 0) v = (r[0].left[1] + 2 * r[0].left[0] + r[0].top[1] + 2) >> 2;
-    else if (e == n0 - 1) v = p[e];
-    else v = (p[e - 1] + 2 * p[e] + p[e + 1] + 2) >> 2;
-    (is_top ? r[0].ftop : r[0].fleft)[e] = (Pix)v;
-  }
-  CTU_SYNC();
+  refs_smooth_dc(log2w, mask, n_of[0], r);
 }
 template <typename Pix> CTU_FN void build_refs(const SmTables *T, const CtuConfig *cfg, CtuWorkT<Pix> *W, LcuLevel<Pix> *L, int log2w, int color, int x, int y, IntraRefs<Pix> *r)
 {

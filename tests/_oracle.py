@@ -671,6 +671,29 @@ class Ref:
                                           type_, scan_mode, tr_skip, P(after))
         return float(bits), after[:self.cabac_ctx_size()].copy()
 
+    def intra_tu(self, qp, lambda_, rdoq, rdoq_skip, signhide, trskip, cabac0, sc, color, log2n, depth, tr_depth, nxn, mode, scan,
+                 alt, top, left, src):
+        """One intra transform unit as the CTU search evaluates it: prediction from the unfiltered references, quantisation
+        (with the transform-skip decision of a 4x4 luma unit when `trskip` and alt < 0; alt 0 / 1 forces an alternative),
+        SSD and the coefficient bits on the search models `sc` -> dict(pred, rec, coeff, has, tr_skip, ssd, bits)."""
+        n = 1 << log2n
+        if not hasattr(self, "_tu_lib"):
+            # oracle/ref_tu.c, a library of its own with an encoder of its own: the call rewrites the configuration's switches
+            so = os.path.join(REF_DIR, "libkvzref_tu.so" if self.pix == np.uint8 else "libkvzref_tu_10b.so")
+            assert os.path.exists(so), f"{so} missing: make -C oracle ref builds it"
+            self._tu_lib = C.CDLL(so)
+            self._tu_lib.kvzref_tu_open.restype = C.c_void_p
+            self._tu_lib.kvzref_intra_tu.restype = C.c_double
+            self._tu_ctx = C.c_void_p(self._tu_lib.kvzref_tu_open())
+            assert self._tu_ctx
+        L = self._tu_lib
+        bufs = dict(cabac0=al(cabac0, np.uint8), sc=al(sc, np.uint8), top=al(top, self.pix), left=al(left, self.pix), src=al(src, self.pix))
+        pred, rec, coeff, oi = aligned(n * n, self.pix), aligned(n * n, self.pix), aligned(n * n, np.int16), aligned(4, np.int32)
+        bits = L.kvzref_intra_tu(self._tu_ctx, qp, C.c_double(lambda_), rdoq, rdoq_skip, signhide, trskip, P(bufs["cabac0"]), P(bufs["sc"]),
+                                 color, log2n, depth, tr_depth, nxn, mode, scan, alt, P(bufs["top"]), P(bufs["left"]), P(bufs["src"]),
+                                 P(pred), P(rec), P(coeff), P(oi))
+        return dict(pred=pred.copy(), rec=rec.copy(), coeff=coeff.copy(), has=int(oi[0]), tr_skip=int(oi[1]), ssd=int(oi[2]), bits=float(bits))
+
     # -- nal
     def array_checksum(self, data, height, width, stride, impl="generic"):
         out = aligned(4, np.uint8)

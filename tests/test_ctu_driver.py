@@ -62,9 +62,9 @@ def _encode(binary, clip, w, h, out, preset, qp, env=None, extra=()):
     return r.stderr
 
 
-def _identity(tmp_path, provider, w, h, frames, preset, qp, noisy=False, extra=(), verify=True):
+def _identity(tmp_path, provider, w, h, frames, preset, qp, noisy=False, extra=(), verify=True, clip=None):
     ref_bin, ctu_bin = _need("kvazaar", "kvazaar_ctu")
-    clip = _clip(tmp_path, w, h, frames, noisy)
+    clip = clip or _clip(tmp_path, w, h, frames, noisy)
     a, b = str(tmp_path / "ref.hevc"), str(tmp_path / "ctu.hevc")
     _encode(ref_bin, clip, w, h, a, preset, qp, extra=extra)
     log = _encode(ctu_bin, clip, w, h, b, preset, qp, env={"KVZ_CTU_PROVIDER": provider}, extra=extra)

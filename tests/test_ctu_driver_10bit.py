@@ -40,9 +40,9 @@ def _clip(tmp_path, w, h, frames, noisy, input_bitdepth):
     return p
 
 
-def _identity10(tmp_path, provider, w, h, frames, preset, qp, noisy=False, input_bitdepth=10, extra=(), verify=True):
+def _identity10(tmp_path, provider, w, h, frames, preset, qp, noisy=False, input_bitdepth=10, extra=(), verify=True, clip=None):
     ref_bin, ctu_bin = _need("kvazaar_10b", "kvazaar_ctu_10b")
-    clip = _clip(tmp_path, w, h, frames, noisy, input_bitdepth)
+    clip = clip or _clip(tmp_path, w, h, frames, noisy, input_bitdepth)
     extra = ("--input-bitdepth", str(input_bitdepth), *extra)
     a, b = str(tmp_path / "ref.hevc"), str(tmp_path / "ctu.hevc")
     _encode(ref_bin, clip, w, h, a, preset, qp, extra=extra)

@@ -6,29 +6,11 @@ import sys, os, tempfile, pathlib, itertools
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, 'tests')); sys.path.insert(0, os.path.join(ROOT, 'tools'))
 import test_ctu_driver as T
-import numpy as np
+from synth_yuv import extreme_pictures
 tmp=pathlib.Path(tempfile.mkdtemp(prefix='kvzn_', dir='/tmp'))
 ref_bin, ctu_bin = [os.path.join(T.REF_DIR,n) for n in ("kvazaar","kvazaar_ctu")]
 w,h=136,72
-r=np.random.default_rng(3)
-yy,xx=np.mgrid[0:h,0:w]
-def planes(y,u=None,v=None):
-    y=np.clip(y,0,255).astype(np.uint8)
-    u=np.full((h//2,w//2),128,np.uint8) if u is None else np.clip(u,0,255).astype(np.uint8)
-    v=np.full((h//2,w//2),128,np.uint8) if v is None else np.clip(v,0,255).astype(np.uint8)
-    return y.tobytes()+u.tobytes()+v.tobytes()
-contents={
- 'flat128': planes(np.full((h,w),128)),
- 'black': planes(np.zeros((h,w)),np.zeros((h//2,w//2)),np.zeros((h//2,w//2))),
- 'white': planes(np.full((h,w),255),np.full((h//2,w//2),255),np.full((h//2,w//2),255)),
- 'checker1': planes(((xx+yy)%2)*255, ((xx[:h//2,:w//2]+yy[:h//2,:w//2])%2)*255, 255-((xx[:h//2,:w//2]+yy[:h//2,:w//2])%2)*255),
- 'vstripes': planes((xx%4<2)*255),
- 'hstripes8': planes((yy%16<8)*200+20),
- 'fullnoise': planes(r.integers(0,256,(h,w)), r.integers(0,256,(h//2,w//2)), r.integers(0,256,(h//2,w//2))),
- 'diag_edge': planes((xx>yy*2)*180+40, (xx[:h//2,:w//2]>yy[:h//2,:w//2])*100+60),
- 'ramp': planes(xx*255//w, yy[:h//2,:w//2]*255//(h//2), xx[:h//2,:w//2]*255//(w//2)),
- 'blocks': planes(((xx//8+yy//8)%2)*120+60+r.integers(-2,3,(h,w))),
-}
+contents=extreme_pictures(w,h)
 bad=0;n=0
 for (name,data),preset,qp in itertools.product(contents.items(),["ultrafast","medium","veryslow"],[12,30,46]):
     clip=str(tmp/f"{name}.yuv"); open(clip,'wb').write(data)

@@ -55,6 +55,34 @@ def noisy_frame_10b(width, height, seed=5, frame_idx=0):
     return np.concatenate([np.clip(np.rint(p), 0, 1023).astype(np.uint16).ravel() for p in (base, u, v)])
 
 
+def extreme_pictures(w, h, bitdepth=8, seed=3):
+    """One 4:2:0 picture of each kind of extreme content -> {name: bytes} (16-bit little-endian samples above 8 bits):
+    flat, black, white, 1-pixel checkerboard, stripes, full-range noise, edges, ramps, blocks.  They drive clipping,
+    all-zero residuals, transform skip and saturated SAO."""
+    m = (1 << bitdepth) - 1
+    k = (m + 1) >> 8
+    r = np.random.default_rng(seed)
+    yy, xx = np.mgrid[0:h, 0:w]
+    cy, cx = yy[:h // 2, :w // 2], xx[:h // 2, :w // 2]
+
+    def planes(y, u=None, v=None):
+        mid = np.full((h // 2, w // 2), 128 * k)
+        out = [np.clip(p, 0, m) for p in (y, mid if u is None else u, mid if v is None else v)]
+        return b"".join((p.astype(np.uint8) if bitdepth == 8 else p.astype("<u2")).tobytes() for p in out)
+    return {
+        "flat128": planes(np.full((h, w), 128 * k)),
+        "black": planes(np.zeros((h, w)), np.zeros((h // 2, w // 2)), np.zeros((h // 2, w // 2))),
+        "white": planes(np.full((h, w), m), np.full((h // 2, w // 2), m), np.full((h // 2, w // 2), m)),
+        "checker1": planes(((xx + yy) % 2) * m, ((cx + cy) % 2) * m, m - ((cx + cy) % 2) * m),
+        "vstripes": planes((xx % 4 < 2) * m),
+        "hstripes8": planes((yy % 16 < 8) * 200 * k + 20 * k),
+        "fullnoise": planes(r.integers(0, m + 1, (h, w)), r.integers(0, m + 1, (h // 2, w // 2)), r.integers(0, m + 1, (h // 2, w // 2))),
+        "diag_edge": planes((xx > yy * 2) * 180 * k + 40 * k, (cx > cy) * 100 * k + 60 * k),
+        "ramp": planes(xx * m // w, cy * m // (h // 2), cx * m // (w // 2)),
+        "blocks": planes(((xx // 8 + yy // 8) % 2) * 120 * k + 60 * k + r.integers(-2 * k, 2 * k + 1, (h, w))),
+    }
+
+
 def frame_fn(noisy=False, bitdepth=8):
     if bitdepth == 10:
         return noisy_frame_10b if noisy else synth_frame_10b
