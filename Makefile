@@ -16,7 +16,7 @@ lib: $(LIB)
 # make PROF=1: the CTU driver with its phase profile (diagnostic; kvz_cuda_ctu_close prints it)
 CTUFLAGS  := $(if $(PROF),-DKVZ_CTU_PROF,)
 
-$(OBJDIR)/ctu_driver.o: $(SRCDIR)/ctu_driver.cu $(wildcard $(SRCDIR)/*.cuh) $(wildcard $(SRCDIR)/ctu/*.h) include/kvz_cuda.h include/kvz_cuda_ctu.h
+$(OBJDIR)/ctu_driver.o: $(SRCDIR)/ctu_driver.cu $(wildcard $(SRCDIR)/*.cuh) $(wildcard $(SRCDIR)/*.h) $(wildcard $(SRCDIR)/ctu/*.h) include/kvz_cuda.h include/kvz_cuda_ctu.h
 	@mkdir -p $(OBJDIR)
 	$(NVCC) $(NVFLAGS) $(CTUFLAGS) -c $< -o $@
 
@@ -24,7 +24,7 @@ $(OBJDIR)/me_search.o: $(SRCDIR)/me_search.cu $(wildcard $(SRCDIR)/*.cuh) $(wild
 	@mkdir -p $(OBJDIR)
 	$(NVCC) $(NVFLAGS) -c $< -o $@
 
-$(OBJDIR)/%.o: $(SRCDIR)/%.cu $(wildcard $(SRCDIR)/*.cuh) include/kvz_cuda.h
+$(OBJDIR)/%.o: $(SRCDIR)/%.cu $(wildcard $(SRCDIR)/*.cuh) $(wildcard $(SRCDIR)/*.h) include/kvz_cuda.h
 	@mkdir -p $(OBJDIR)
 	$(NVCC) $(NVFLAGS) -c $< -o $@
 
@@ -37,9 +37,9 @@ $(LIB): $(OBJS)
 PROBE     := tests/cuda/libkvzctu_probe.so
 PROBE_HOST := tests/hostsim/libkvzctu_probe_host.so
 probe: $(PROBE) $(PROBE_HOST)
-$(PROBE): tests/cuda/ctu_tu_probe.cu $(wildcard $(SRCDIR)/ctu/*.h)
+$(PROBE): tests/cuda/ctu_tu_probe.cu $(wildcard $(SRCDIR)/*.h) $(wildcard $(SRCDIR)/ctu/*.h)
 	$(NVCC) $(ARCH) -O3 -std=c++17 -fmad=false -Xcompiler -fPIC,-Wall -shared -o $@ $< -lcudart
-$(PROBE_HOST): tests/cuda/ctu_tu_probe.cu $(wildcard $(SRCDIR)/ctu/*.h)
+$(PROBE_HOST): tests/cuda/ctu_tu_probe.cu $(wildcard $(SRCDIR)/*.h) $(wildcard $(SRCDIR)/ctu/*.h)
 	g++ -O2 -g -std=c++17 -fPIC -shared -ffp-contract=off -Wall -Wno-unused-function -Wno-unknown-pragmas -x c++ -o $@ $<
 
 oracle:

@@ -3,163 +3,42 @@
 // kvz_encode_coeff_nxn in only_count mode (src/strategies/generic/encode_coding_tree-generic.c:40-290) together with
 // kvz_encode_last_significant_xy (src/encode_coding_tree.c:63-115) and kvz_cabac_write_coeff_remain (src/cabac.c:275-301).
 //
-// Counting mode adds kvz_f_entropy_bits[state ^ bin] (= kvz_entropy_bits / 2^15, exact in float and double) per
-// context-coded bin and 1 per bypass bin, in coding order, into two double accumulators (last position, the rest) that
-// are added at the end -- reproduced here in that order.  With `update` the context models adapt inside the TU
-// exactly as CABAC_BIN would (state transition tables of the standard); every TU of a batch starts from the same
-// context image.  One thread per TU.
+// The count itself is coeff_bits (coeff_rules.h), in units of 2^-15 bit.  With `update` the context models adapt
+// inside the TU exactly as CABAC_BIN would; every TU of a batch starts from the same context image.  One thread per TU,
+// or (16x16 and 32x32 grids, no adaptation) one warp per TU.
 #include "rdoq.cuh"
 
 namespace kvzc {
 
-// CABAC state transition on the packed state byte (state << 1 | mps): kvz_g_auc_next_state_mps / _lps (cabac.c:40-62)
-__device__ __forceinline__ uint8_t cabac_next_mps(uint8_t uc) { return uc < 124 ? (uint8_t)(uc + 2) : uc; }
-__device__ __forceinline__ uint8_t cabac_next_lps(uint8_t uc)
-{
-  const uint8_t trans[64] = { 0, 0, 1, 2, 2, 4, 4, 5, 6, 7, 8, 9, 9, 11, 11, 12, 13, 13, 15, 15, 16, 16, 18, 18, 19, 19, 21, 21, 22, 22, 23, 24,
-                              24, 25, 26, 26, 27, 27, 28, 29, 29, 30, 30, 30, 31, 32, 32, 33, 33, 33, 34, 34, 35, 35, 35, 36, 36, 36, 37, 37, 37, 38, 38, 63 };
-  const int s = uc >> 1, mps = uc & 1;
-  return (uint8_t)((trans[s] << 1) | (s == 0 ? 1 - mps : mps));
-}
-
-struct CostCtx {
+// coeff_bits' policy: scans computed, entropy bits staged in shared memory (rdoq_load_ebits), the models of this TU
+struct CostWalk {
   uint8_t *models;            // this TU's (possibly private) context image
-  const int32_t *eb;          // entropy-bit table (rdoq_load_ebits)
-  bool update;
-  // CABAC_FBITS_UPDATE (cabac.h:133-139)
-  __device__ __forceinline__ void bin(double &bits, int model_off, int val)
+  const int32_t *eb;
+  bool update, trskip, sh;
+  int32_t abs_coeff[16];
+  struct Scan { int scan_idx, log2n; __device__ int operator[](int i) const { return scan_pos(scan_idx, log2n, i); } };
+  struct ScanCg {
+    int scan_idx, log2n;
+    __device__ int operator[](int i) const
+    {
+      const int first = scan_pos(scan_idx, log2n, i << 4), n = 1 << log2n;
+      return ((first >> log2n) >> 2) * (n >> 2) + ((first & (n - 1)) >> 2);
+    }
+  };
+  __device__ Scan scan(int scan_idx, int log2n) const { return Scan{ scan_idx, log2n }; }
+  __device__ ScanCg scan_cg(int scan_idx, int log2n) const { return ScanCg{ scan_idx, log2n }; }
+  __device__ int group_idx(int x) const { return last_group(x); }
+  __device__ SigCtx4 sig_ctx4() const { return SigCtx4(); }
+  __device__ int32_t *abs_scratch() { return abs_coeff; }
+  __device__ bool trskip_enable() const { return trskip; }
+  __device__ bool signhide() const { return sh; }
+  __device__ void bin(int off, int val, long long *bits)
   {
-    const uint8_t st = models[model_off];
-    bits += (double)eb[st ^ val] * (1.0 / 32768.0);
-    if (update) models[model_off] = ((st & 1) == val) ? cabac_next_mps(st) : cabac_next_lps(st);
+    const uint8_t st = models[off];
+    *bits += eb[st ^ val];
+    if (update) models[off] = ((st & 1) == val) ? cabac_next_mps(st) : cabac_next_lps(st);
   }
 };
-
-#define CTX_OFF(member) ((int)offsetof(kvz_cuda_cabac_ctx, member))
-
-// bits of coeff_abs_level_remaining (cabac.c:275-301)
-__device__ __forceinline__ int coeff_remain_bits(int symbol, int rice)
-{
-  if (symbol < (3 << rice)) return (symbol >> rice) + 1 + rice;
-  int length = rice;
-  symbol -= 3 << rice;
-  while (symbol >= (1 << length)) { symbol -= 1 << length; ++length; }
-  return 3 + length + 1 - rice + length;
-}
-
-__device__ double coeff_cost_tu(CostCtx &c, const int16_t *coeff, int log2n, int type, int scan_idx, int trskip_enable, int tr_skip, int signhide)
-{
-  const int n = 1 << log2n, side = n >> 2, ncg = side * side;
-  uint64_t cg_flags = 0;                                                // sig_coeffgroup_flag, bit = cg_y * side + cg_x
-  for (int g = 0; g < ncg; ++g) {
-    const int gy = g / side, gx = g - gy * side;
-    bool any = false;
-    for (int r = 0; r < 4 && !any; ++r) {
-      const int16_t *row = coeff + (gy * 4 + r) * n + gx * 4;
-      any = (row[0] | row[1] | row[2] | row[3]) != 0;
-    }
-    if (any) cg_flags |= 1ull << g;
-  }
-  if (!cg_flags) return 0.0;                                            // get_coeff_cabac_cost: no coefficients -> 0 (rdo.c:231-238)
-  auto cg_of_scan = [&](int i) { const int first = scan_pos(scan_idx, log2n, i << 4); return ((first >> log2n) >> 2) * side + ((first & (n - 1)) >> 2); };
-  int cg_last = ncg - 1;
-  while (!((cg_flags >> cg_of_scan(cg_last)) & 1)) --cg_last;
-  int scan_last = cg_last * 16 + 15;
-  while (!coeff[scan_pos(scan_idx, log2n, scan_last)]) --scan_last;
-  const int pos_last = scan_pos(scan_idx, log2n, scan_last);
-
-  double bits = 0;                                                      // encode_coeff_nxn's accumulator
-  if (n == 4 && trskip_enable) c.bin(bits, type == 0 ? CTX_OFF(transform_skip_model_luma) : CTX_OFF(transform_skip_model_chroma), tr_skip);
-
-  // last significant position (encode_coding_tree.c:63-115), its own accumulator
-  double bits_last = 0;
-  {
-    int lx = pos_last & (n - 1), ly = pos_last >> log2n;
-    if (scan_idx == 2) { const int t = lx; lx = ly; ly = t; }
-    const int idx = log2n - 2;
-    const int ctx_offset = type ? 0 : (idx * 3 + (idx + 1) / 4);
-    const int shift = type ? idx : (idx + 3) / 4;
-    const int base_x = type ? CTX_OFF(cu_ctx_last_x_chroma) : CTX_OFF(cu_ctx_last_x_luma);
-    const int base_y = type ? CTX_OFF(cu_ctx_last_y_chroma) : CTX_OFF(cu_ctx_last_y_luma);
-    const int gx = last_group(lx), gy = last_group(ly), gmax = last_group(n - 1);
-    for (int k = 0; k < gx; ++k) c.bin(bits_last, base_x + ctx_offset + (k >> shift), 1);
-    if (gx < gmax) c.bin(bits_last, base_x + ctx_offset + (gx >> shift), 0);
-    for (int k = 0; k < gy; ++k) c.bin(bits_last, base_y + ctx_offset + (k >> shift), 1);
-    if (gy < gmax) c.bin(bits_last, base_y + ctx_offset + (gy >> shift), 0);
-    if (gx > 3) bits_last += (gx - 2) / 2;
-    if (gy > 3) bits_last += (gy - 2) / 2;
-  }
-
-  const int base_cg = CTX_OFF(cu_sig_coeff_group_model) + type;
-  const int base_sig = type == 0 ? CTX_OFF(cu_sig_model_luma) : CTX_OFF(cu_sig_model_chroma);
-  int c1 = 1;
-  int scan_pos_sig = scan_last;
-  for (int i = cg_last; i >= 0; --i) {
-    const int sub_pos = i << 4;
-    int abs_coeff[16];
-    const int cg_blk = cg_of_scan(i);
-    const int cgy = cg_blk / side, cgx = cg_blk - cgy * side;
-    int last_nz = -1, first_nz = 16, num_nz = 0, rice = 0;
-    if (scan_pos_sig == scan_last) {
-      abs_coeff[0] = abs((int)coeff[pos_last]);
-      num_nz = 1; last_nz = scan_pos_sig; first_nz = scan_pos_sig;
-      --scan_pos_sig;
-    }
-    const int right = (cgx < side - 1) ? (int)((cg_flags >> (cgy * side + cgx + 1)) & 1) : 0;
-    const int lower = (cgy < side - 1) ? (int)((cg_flags >> ((cgy + 1) * side + cgx)) & 1) : 0;
-    if (i == cg_last || i == 0) cg_flags |= 1ull << cg_blk;
-    else c.bin(bits, base_cg + (right || lower), (int)((cg_flags >> cg_blk) & 1));
-    if ((cg_flags >> cg_blk) & 1) {
-      const int pattern = (n == 4) ? -1 : right + (lower << 1);
-      for (; scan_pos_sig >= sub_pos; --scan_pos_sig) {
-        const int blk = scan_pos(scan_idx, log2n, scan_pos_sig);
-        const int sig = coeff[blk] != 0;
-        if (scan_pos_sig > sub_pos || i == 0 || num_nz)
-          c.bin(bits, base_sig + rdoq_sig_ctx(pattern, scan_idx, blk & (n - 1), blk >> log2n, log2n, type), sig);
-        if (sig) {
-          abs_coeff[num_nz++] = abs((int)coeff[blk]);
-          if (last_nz == -1) last_nz = scan_pos_sig;
-          first_nz = scan_pos_sig;
-        }
-      }
-    } else {
-      scan_pos_sig = sub_pos - 1;
-    }
-    if (num_nz > 0) {
-      const bool sign_hidden = last_nz - first_nz >= 4;
-      int ctx_set = (i > 0 && type == 0) ? 2 : 0;
-      if (c1 == 0) ++ctx_set;
-      c1 = 1;
-      const int base_one = (type == 0 ? CTX_OFF(cu_one_model_luma) : CTX_OFF(cu_one_model_chroma)) + 4 * ctx_set;
-      const int num_c1 = min(num_nz, 8);
-      int first_c2 = -1;
-      for (int k = 0; k < num_c1; ++k) {
-        const int symbol = abs_coeff[k] > 1;
-        c.bin(bits, base_one + c1, symbol);
-        if (symbol) { c1 = 0; if (first_c2 == -1) first_c2 = k; }
-        else if (c1 < 3 && c1 > 0) ++c1;
-      }
-      if (c1 == 0 && first_c2 != -1)
-        c.bin(bits, (type == 0 ? CTX_OFF(cu_abs_model_luma) : CTX_OFF(cu_abs_model_chroma)) + ctx_set, abs_coeff[first_c2] > 2);
-      bits += (signhide && sign_hidden) ? num_nz - 1 : num_nz;             // sign bins (bypass)
-      if (c1 == 0 || num_nz > 8) {
-        int first_coeff2 = 1;
-        for (int k = 0; k < num_nz; ++k) {
-          const int base_level = (k < 8) ? (2 + first_coeff2) : 1;
-          if (abs_coeff[k] >= base_level) {
-            bits += coeff_remain_bits(abs_coeff[k] - base_level, rice);
-            if (abs_coeff[k] > 3 * (1 << rice)) rice = min(rice + 1, 4);
-          }
-          if (abs_coeff[k] >= 2) first_coeff2 = 0;
-        }
-      }
-    }
-  }
-  double total = 0;
-  total += bits_last;
-  total += bits;
-  return total;
-}
 
 __global__ void __launch_bounds__(128) coeff_cost_kernel(kvz_cuda_coeff_cost_params p, const kvz_cuda_cabac_ctx *__restrict__ cabac,
                                                          const int16_t *__restrict__ coeff, int n, const kvz_cuda_rdoq_tu *__restrict__ tus,
@@ -174,11 +53,12 @@ __global__ void __launch_bounds__(128) coeff_cost_kernel(kvz_cuda_coeff_cost_par
   if (t >= count) return;
   const kvz_cuda_rdoq_tu tu = tus[t];
   kvz_cuda_cabac_ctx mine;                       // private copy only when the models adapt
-  CostCtx c;
-  c.eb = s_ebits; c.update = p.update != 0;
+  CostWalk c;
+  c.eb = s_ebits; c.update = p.update != 0; c.trskip = p.trskip_enable != 0; c.sh = p.signhide_enable != 0;
   if (c.update) { mine = s_ctx; c.models = (uint8_t *)&mine; } else c.models = (uint8_t *)&s_ctx;
   const int log2n = 31 - __clz(n);
-  bits_out[t] = coeff_cost_tu(c, coeff + tu.off_coef, log2n, tu.type, tu.scan_idx, p.trskip_enable, tu.block_type /* tr_skip flag */, p.signhide_enable);
+  const long long bits = coeff_bits(c, coeff + tu.off_coef, log2n, tu.type, tu.scan_idx, tu.block_type /* tr_skip flag */, COEFF_NO_MASK);
+  bits_out[t] = (double)bits * (1.0 / 32768.0);
   if (c.update && ctx_out) ctx_out[t] = mine;
 }
 
@@ -200,16 +80,16 @@ __global__ void __launch_bounds__(128) coeff_cost_grid_kernel(int signhide, int 
   const int w = 1 << log2n;
   int scan = 0;
   if ((!is_chroma && w <= 8) || (is_chroma && w == 4)) { const int m = modes[t]; scan = (m >= 6 && m <= 14) ? 2 : ((m >= 22 && m <= 30) ? 1 : 0); }
-  CostCtx c;
-  c.eb = s_ebits; c.update = false; c.models = (uint8_t *)&s_ctx;
-  bits_out[t] = coeff_cost_tu(c, coeff + (size_t)t * w * w, log2n, is_chroma ? 2 : 0, scan, trskip_enable, 0, signhide);   // the flag is counted as 0 (rdo.c:251-258)
+  CostWalk c;
+  c.eb = s_ebits; c.update = false; c.trskip = trskip_enable != 0; c.sh = signhide != 0; c.models = (uint8_t *)&s_ctx;
+  const long long bits = coeff_bits(c, coeff + (size_t)t * w * w, log2n, is_chroma ? 2 : 0, scan, 0, COEFF_NO_MASK);   // the flag is counted as 0 (rdo.c:251-258)
+  bits_out[t] = (double)bits * (1.0 / 32768.0);
 }
 
 
 // ---- warp per TU, no context adaptation (16x16 and 32x32 grids) -------------------------------------------------------
-// Without adaptation every term of the count is an integer number of 1/32768 bits (kvz_f_entropy_bits = integers / 2^15,
-// bypass bins = 1), so the reference's double accumulators are exact at every step and the total does not depend on
-// the order of the additions: total = (sum of integer costs) / 2^15.  That makes the count position-parallel:
+// The count is exact in units of 2^-15 bit (coeff_bits), so the total does not depend on the order of the additions.
+// Without adaptation that makes it position-parallel:
 //   * a lane owns coefficient groups (scan index i = lane, lane + 32): non-zero mask, coefficient magnitudes in coding
 //     order, whether one of its first eight magnitudes exceeds 1 (the only state a group hands to the next one:
 //     "c1 == 0" selects the next group's context set);
@@ -221,6 +101,8 @@ __device__ long long coeff_cost_tu_warp(const uint8_t *models, const int32_t *eb
 {
   const int n = 1 << log2n, side = n >> 2, ncg = side * side;
   auto cost = [&](int model_off, int val) { return (long long)eb[models[model_off] ^ val]; };
+  CostWalk w;
+  w.models = (uint8_t *)models; w.eb = eb; w.update = false;
   // pass 1: per group (scan order, diagonal: scan_idx is 0 for these sizes) the non-zero mask in coding order
   int my_abs[2][16];
   unsigned my_mask[2] = { 0, 0 };
@@ -233,7 +115,7 @@ __device__ long long coeff_cost_tu_warp(const uint8_t *models, const int32_t *eb
     const int by = (first >> log2n) & ~3, bx = (first & (n - 1)) & ~3;
 #pragma unroll
     for (int k = 0; k < 16; ++k) {
-      const int in = scan_pos_small(0, 2, k);                             // position inside the 4x4 group
+      const int in = scan_small(0, 2, k);                             // position inside the 4x4 group
       const int v = coeff[(by + (in >> 2)) * n + bx + (in & 3)];
       my_abs[r][k] = abs(v);
       if (v) my_mask[r] |= 1u << k;
@@ -258,24 +140,11 @@ __device__ long long coeff_cost_tu_warp(const uint8_t *models, const int32_t *eb
   auto flag_at = [&](int cgx, int cgy) { return s_raster[cgy * side + cgx] != 0; };
   long long sum = 0;
   if (lane == 0) {
-    // last significant position (encode_coding_tree.c:63-115)
     const int pos_last = scan_pos(0, log2n, scan_last);
-    const int lx = pos_last & (n - 1), ly = pos_last >> log2n;
-    const int idx = log2n - 2;
-    const int ctx_offset = type ? 0 : (idx * 3 + (idx + 1) / 4);
-    const int shift = type ? idx : (idx + 3) / 4;
-    const int base_x = type ? CTX_OFF(cu_ctx_last_x_chroma) : CTX_OFF(cu_ctx_last_x_luma);
-    const int base_y = type ? CTX_OFF(cu_ctx_last_y_chroma) : CTX_OFF(cu_ctx_last_y_luma);
-    const int gx = last_group(lx), gy = last_group(ly), gmax = last_group(n - 1);
-    for (int k = 0; k < gx; ++k) sum += cost(base_x + ctx_offset + (k >> shift), 1);
-    if (gx < gmax) sum += cost(base_x + ctx_offset + (gx >> shift), 0);
-    for (int k = 0; k < gy; ++k) sum += cost(base_y + ctx_offset + (k >> shift), 1);
-    if (gy < gmax) sum += cost(base_y + ctx_offset + (gy >> shift), 0);
-    if (gx > 3) sum += 32768ll * ((gx - 2) / 2);
-    if (gy > 3) sum += 32768ll * ((gy - 2) / 2);
+    sum += last_pos_bits(w, pos_last & (n - 1), pos_last >> log2n, n, log2n, type);
   }
-  const int base_cg = CTX_OFF(cu_sig_coeff_group_model) + type;
-  const int base_sig = type == 0 ? CTX_OFF(cu_sig_model_luma) : CTX_OFF(cu_sig_model_chroma);
+  const int base_cg = CTX_SIG_CG + type;
+  const int base_sig = type == 0 ? CTX_SIG_LUMA : CTX_SIG_CHROMA;
   for (int r = 0; r < 2; ++r) {
     const int i = lane + 32 * r;
     if (i >= ncg || i > cg_last) continue;
@@ -295,8 +164,8 @@ __device__ long long coeff_cost_tu_warp(const uint8_t *models, const int32_t *eb
     for (int k = top; k >= 0; --k) {
       const bool earlier_nz = (mask >> (k + 1)) != 0;                      // a non-zero coefficient coded before this one in the group
       if (k > 0 || i == 0 || earlier_nz) {
-        const int in = scan_pos_small(0, 2, k);
-        sum += cost(base_sig + rdoq_sig_ctx(pattern, 0, bx + (in & 3), by + (in >> 2), log2n, type), (mask >> k) & 1);
+        const int in = scan_small(0, 2, k);
+        sum += cost(base_sig + sig_ctx_inc(SigCtx4(), pattern, 0, bx + (in & 3), by + (in >> 2), log2n, type), (mask >> k) & 1);
       }
     }
     if (!mask) continue;
@@ -313,7 +182,7 @@ __device__ long long coeff_cost_tu_warp(const uint8_t *models, const int32_t *eb
       break;
     }
     int c1 = 1, first_c2 = -1;
-    const int base_one = (type == 0 ? CTX_OFF(cu_one_model_luma) : CTX_OFF(cu_one_model_chroma)) + 4 * ctx_set;
+    const int base_one = (type == 0 ? CTX_ONE_LUMA : CTX_ONE_CHROMA) + 4 * ctx_set;
     const int num_c1 = min(num_nz, 8);
     for (int k = 0; k < num_c1; ++k) {
       const int symbol = abs_c[k] > 1;
@@ -321,7 +190,7 @@ __device__ long long coeff_cost_tu_warp(const uint8_t *models, const int32_t *eb
       if (symbol) { c1 = 0; if (first_c2 == -1) first_c2 = k; }
       else if (c1 < 3 && c1 > 0) ++c1;
     }
-    if (c1 == 0 && first_c2 != -1) sum += cost((type == 0 ? CTX_OFF(cu_abs_model_luma) : CTX_OFF(cu_abs_model_chroma)) + ctx_set, abs_c[first_c2] > 2);
+    if (c1 == 0 && first_c2 != -1) sum += cost((type == 0 ? CTX_ABS_LUMA : CTX_ABS_CHROMA) + ctx_set, abs_c[first_c2] > 2);
     sum += 32768ll * ((signhide && last_nz - first_nz >= 4) ? num_nz - 1 : num_nz);
     if (c1 == 0 || num_nz > 8) {
       int first_coeff2 = 1, rice = 0;

@@ -14,6 +14,7 @@
 #include <stdint.h>
 #include <stddef.h>
 #include <string.h>
+#include "../coeff_rules.h"
 
 #if defined(__CUDACC__)
 #define CTU_FN __device__ __forceinline__
@@ -78,6 +79,8 @@ enum { PR_LOAD, PR_SEARCH, PR_STORE, PR_DEBLOCK, PR_SAO, PR_TRACK, PR_REFS, PR_S
 #endif
 
 namespace kvzctu {
+
+using namespace kvzcoeff;
 
 // ---------------------------------------------------------------------------------------------- sample type
 // The algorithm is compiled once per sample type: uint8_t for 8-bit, uint16_t for 10-bit pictures (kvz_pixel of the
@@ -170,16 +173,7 @@ CTU_FN int zorder(int width, int x, int y)
 }
 
 // ---------------------------------------------------------------------------------------------- CABAC models
-// Memory image of cabac_data_t.ctx (ref: src/cabac.h:66-102), same member order as kvz_cuda_cabac_ctx.
-enum CtxOff {
-  CTX_SAO_MERGE = 0, CTX_SAO_TYPE = 1, CTX_SPLIT = 2, CTX_INTRA_MODE = 5, CTX_CHROMA_PRED = 6, CTX_INTER_DIR = 8,
-  CTX_TRANS_SUBDIV = 13, CTX_CBF_LUMA = 16, CTX_CBF_CHROMA = 20, CTX_QP_DELTA = 24, CTX_PART_SIZE = 28,
-  CTX_SIG_CG = 32, CTX_SIG_LUMA = 36, CTX_SIG_CHROMA = 63, CTX_LAST_Y_LUMA = 78, CTX_LAST_Y_CHROMA = 93,
-  CTX_LAST_X_LUMA = 108, CTX_LAST_X_CHROMA = 123, CTX_ONE_LUMA = 138, CTX_ONE_CHROMA = 154, CTX_ABS_LUMA = 162,
-  CTX_ABS_CHROMA = 166, CTX_PRED_MODE = 168, CTX_SKIP_FLAG = 169, CTX_MERGE_IDX = 172, CTX_MERGE_FLAG = 173,
-  CTX_TQ_BYPASS = 174, CTX_MVD = 175, CTX_REF_PIC = 177, CTX_MVP_IDX = 179, CTX_ROOT_CBF = 181,
-  CTX_TRSKIP_LUMA = 182, CTX_TRSKIP_CHROMA = 183, CTX_COUNT = 184
-};
+// The models as a memory image of cabac_data_t.ctx (offsets: CtxOff, coeff_rules.h).
 struct alignas(16) CabacState {     // 192 bytes: copied around every speculative branch, as 16-byte moves
   uint8_t ctx[CTX_COUNT];
   uint8_t update;          // cabac_data_t.update travels with every copy of the struct (ref: search.c:655, 956-958)
@@ -212,18 +206,6 @@ struct CtuTables {
 
 // ---- host-side table construction (product host code and the test build share it)
 namespace tables_detail {
-inline int scan_small(int scan_idx, int dim_log2, int idx)
-{
-  const int dim = 1 << dim_log2;
-  if (scan_idx == 1) return idx;
-  if (scan_idx == 2) return (idx & (dim - 1)) * dim + (idx >> dim_log2);
-  int d = 0, start = 0;
-  for (;; ++d) {
-    const int ylo = d - (dim - 1) > 0 ? d - (dim - 1) : 0, yhi = d < dim - 1 ? d : dim - 1, len = yhi - ylo + 1;
-    if (idx < start + len) { const int y = yhi - (idx - start); return y * dim + (d - y); }
-    start += len;
-  }
-}
 inline int zidx16(int ux, int uy)
 {
   int z = 0;
@@ -277,40 +259,21 @@ inline void ctu_tables_init(CtuTables *t)
   }
   static const int8_t dst[16] = { 29, 55, 74, 84, 74, 74, 0, -74, 84, -29, -74, 55, 55, -84, 74, -29 };
   memcpy(t->dst4, dst, 16);
-  static const int32_t mps[64] = {
-    32768, 30426, 28306, 26378, 24617, 23005, 21523, 20159, 18899, 17734, 16653, 15650, 14717, 13849, 13038, 12282,
-    11575, 10914, 10294, 9714, 9169, 8658, 8178, 7727, 7303, 6903, 6527, 6173, 5840, 5525, 5228, 4948,
-    4684, 4435, 4199, 3977, 3767, 3568, 3380, 3202, 3034, 2876, 2725, 2583, 2448, 2321, 2200, 2086,
-    1978, 1875, 1778, 1686, 1599, 1517, 1439, 1364, 1294, 1228, 1165, 1105, 1048, 994, 943, 895 };
-  static const int32_t lps[64] = {
-    32768, 35232, 37696, 40159, 42623, 45087, 47551, 50015, 52479, 54942, 57406, 59870, 62334, 64798, 67262, 69725,
-    72189, 74653, 77117, 79581, 82044, 84508, 86972, 89436, 91900, 94363, 96827, 99291, 101755, 104219, 106683, 109146,
-    111610, 114074, 116538, 119002, 121465, 123929, 126393, 128857, 131321, 133785, 136248, 138712, 141176, 143640, 146104, 148568,
-    151031, 153495, 155959, 158423, 160887, 163351, 165814, 168278, 170742, 173207, 175669, 178134, 180598, 183061, 185525, 187989 };
+  static const int32_t mps[64] = { COEFF_EBITS_MPS }, lps[64] = { COEFF_EBITS_LPS };
   for (int i = 0; i < 128; ++i) t->ebits[i] = (i & 1) ? lps[i >> 1] : mps[i >> 1];
-  // state transitions of the standard (table 9-41) on the packed byte (pStateIdx << 1 | valMps)
-  static const uint8_t trans_lps[64] = { 0, 0, 1, 2, 2, 4, 4, 5, 6, 7, 8, 9, 9, 11, 11, 12, 13, 13, 15, 15, 16, 16, 18, 18, 19, 19, 21, 21, 22, 22, 23, 24,
-                                         24, 25, 26, 26, 27, 27, 28, 29, 29, 30, 30, 30, 31, 32, 32, 33, 33, 33, 34, 34, 35, 35, 35, 36, 36, 36, 37, 37, 37, 38, 38, 63 };
   for (int uc = 0; uc < 128; ++uc) {
-    const int s = uc >> 1, m = uc & 1;
-    t->next_mps[uc] = (uint8_t)(uc < 124 ? uc + 2 : uc);
-    t->next_lps[uc] = (uint8_t)((trans_lps[s] << 1) | (s == 0 ? 1 - m : m));
+    t->next_mps[uc] = cabac_next_mps(uc);
+    t->next_lps[uc] = cabac_next_lps(uc);
   }
-  static const uint8_t map4[16] = { 0, 1, 4, 5, 2, 3, 4, 5, 6, 6, 8, 8, 7, 7, 8, 8 };
+  static const uint8_t map4[16] = { COEFF_SIG_CTX4 };
   memcpy(t->sig_ctx4, map4, 16);
-  for (int x = 0; x < 32; ++x) {
-    int g;
-    if (x < 4) g = x; else { int l = 31 - __builtin_clz(x); g = 2 * l + ((x >> (l - 1)) & 1); }
-    t->group_idx[x] = (uint8_t)g;
-  }
-  static const uint8_t mig[10] = { 0, 1, 2, 3, 4, 6, 8, 12, 16, 24 };
+  for (int x = 0; x < 32; ++x) t->group_idx[x] = (uint8_t)last_group(x);
+  static const uint8_t mig[10] = { COEFF_MIN_IN_GROUP };
   memcpy(t->min_in_group, mig, 10);
 }
 
 // ---------------------------------------------------------------------------------------------- small helpers
-CTU_FN int imin(int a, int b) { return a < b ? a : b; }
 CTU_FN int imax(int a, int b) { return a > b ? a : b; }
-CTU_FN int iabs(int a) { return a < 0 ? -a : a; }
 CTU_FN int iclip(int lo, int hi, int v) { return v < lo ? lo : (v > hi ? hi : v); }
 
 // kvz_get_scan_order (ref: src/encoderstate.c:1761-1775), CU_INTRA only
@@ -323,17 +286,8 @@ CTU_FN int scan_order_intra(int mode, int depth)
   return 0;
 }
 
-// kvz_get_scaled_qp (ref: src/transform.c:56-62, 88-102), 8-bit (qp_offset 0)
-CTU_FN int scaled_qp(int type, int qp)
-{
-  if (type == 0) return qp;
-  int q = qp < 0 ? 0 : (qp > 57 ? 57 : qp);
-  if (q < 30) return q;
-  if (q >= 44) return q - 6;
-  const int mid[14] = { 29, 30, 31, 32, 33, 33, 34, 34, 35, 35, 36, 36, 37, 37 };
-  return mid[q - 30];
-}
-// the same with the qp_offset of the bit depth, 6 * (bd - 8) (ref: quant-generic.c:57, 305; rdo.c:672)
-template <typename Pix> CTU_FN int scaled_qp_px(int type, int qp) { return scaled_qp(type, qp) + 6 * (PixDepth<Pix>::bd - 8); }
+// kvz_get_scaled_qp with the qp_offset of the bit depth, 6 * (bd - 8) (ref: quant-generic.c:57, 305; rdo.c:672); the
+// search's QP is never negative, so the offset can be added after the chroma mapping
+template <typename Pix> CTU_FN int scaled_qp_px(int type, int qp) { return scaled_qp(type, qp, 0) + 6 * (PixDepth<Pix>::bd - 8); }
 
 }  // namespace kvzctu

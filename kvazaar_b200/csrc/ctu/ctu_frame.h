@@ -248,7 +248,7 @@ template <typename Pix> CTU_FN_NOINLINE void ctu_deblock(const CtxT<Pix> &c, con
   const int scale = 1 << (PixDepth<Pix>::bd - 8);          // bitdepth_scale (ref: filter.c:373, 590)
   const int beta = dbk_beta(iclip(0, 51, qp + 2 * cfg->deblock_beta)) * scale;
   const int tc_l = dbk_tc(iclip(0, 53, qp + 2 + 2 * cfg->deblock_tc)) * scale;
-  const int tc_c = dbk_tc(iclip(0, 53, scaled_qp(2, qp) + 2 + 2 * cfg->deblock_tc)) * scale;
+  const int tc_c = dbk_tc(iclip(0, 53, scaled_qp(2, qp, 0) + 2 + 2 * cfg->deblock_tc)) * scale;
   const int ux_n = (end_x - x0) / 8, uy_n = (end_y - y0) / 8;
   // pass 1: vertical edges of every 8x8 unit: two luma parts per unit, one chroma part where x % 16 == 0
   #pragma unroll 1

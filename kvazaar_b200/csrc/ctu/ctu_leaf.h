@@ -584,8 +584,6 @@ CTU_FN_NOINLINE void inv_pass(const Team &tm, const int16_t *src, int16_t *dst, 
 CTU_FN int ilog2(int n) { int l = 0; while ((1 << l) < n) ++l; return l; }
 
 // ------------------------------------------------------------------------------------------------ quantisation
-CTU_FN int quant_scale(int r) { const int t[6] = { 26214, 23302, 20560, 18396, 16384, 14564 }; return t[r]; }
-CTU_FN int inv_quant_scale(int r) { const int t[6] = { 40, 45, 51, 57, 64, 72 }; return t[r]; }
 
 // sign-bit hiding of kvz_quant for one coefficient group (ref: quant-generic.c:84-176)
 CTU_FN void quant_sign_hide_group(const SmTables *T, const int16_t *coef, int16_t *q, const int32_t *delta_u, const int32_t *cg_nz,
@@ -682,102 +680,10 @@ CTU_FN_NOINLINE void dequant_block(const Team &tm, const CtuConfig *cfg, const T
 }
 
 // ------------------------------------------------------------------------------------------------ RDOQ
-#define CTU_RDOQ_ONE_BIT (1 << 15)
-struct RdoqModels { const uint8_t *sig, *one, *abs, *cg, *last_x, *last_y, *cbf; const int32_t *eb; uint8_t root_cbf; };
-#define rq_ebits(st, bin) (m.eb[(st) ^ (bin)])
-
-CTU_FN int rdoq_level_rate(const RdoqModels &m, uint32_t abs_level, int ctx_one, int ctx_abs, int rice, uint32_t c1_idx, uint32_t c2_idx)
-{
-  int rate = CTU_RDOQ_ONE_BIT;
-  const uint32_t base_level = (c1_idx < 8) ? (2 + (c2_idx < 1)) : 1;
-  if (abs_level >= base_level) {
-    int symbol = (int)(abs_level - base_level);
-    if (symbol < (3 << rice)) {
-      rate += ((symbol >> rice) + 1 + rice) * CTU_RDOQ_ONE_BIT;
-    } else {
-      int length = rice;
-      symbol -= 3 << rice;
-      while (symbol >= (1 << length)) symbol -= 1 << (length++);
-      rate += (3 + length + 1 - rice + length) * CTU_RDOQ_ONE_BIT;
-    }
-    if (c1_idx < 8) {
-      rate += rq_ebits(m.one[ctx_one], 1);
-      if (c2_idx < 1) rate += rq_ebits(m.abs[ctx_abs], 1);
-    }
-  } else if (abs_level == 1) {
-    rate += rq_ebits(m.one[ctx_one], 0);
-  } else if (abs_level == 2) {
-    rate += rq_ebits(m.one[ctx_one], 1);
-    rate += rq_ebits(m.abs[ctx_abs], 0);
-  }
-  return rate;
-}
-
-// context increment of sig_coeff_flag (ref: context.c:366-397)
-CTU_FN int sig_ctx_inc(const SmTables *T, int pattern, int scan_idx, int px, int py, int log2n, int type)
-{
-  if (px + py == 0) return 0;
-  if (log2n == 2) return T->sig_ctx4[4 * py + px];
-  const int offset = (log2n == 3) ? (scan_idx == 0 ? 9 : 15) : (type == 0 ? 21 : 12);
-  const int sx = px & 3, sy = py & 3;
-  int cnt;
-  if (pattern == 0) cnt = (sx + sy <= 2) ? ((sx + sy == 0) ? 2 : 1) : 0;
-  else if (pattern == 1) cnt = (sy <= 1) ? ((sy == 0) ? 2 : 1) : 0;
-  else if (pattern == 2) cnt = (sx <= 1) ? ((sx == 0) ? 2 : 1) : 0;
-  else cnt = 2;
-  return ((type == 0 && ((px >> 2) + (py >> 2)) > 0) ? 3 : 0) + offset + cnt;
-}
-
-// kvz_rdoq_sign_hiding (ref: rdo.c:518-653); serial, one thread
+// kvz_rdoq_sign_hiding on the unit's rate tables (a call of its own: RDOQ's lanes wait while the leader runs it)
 template <typename Pix> CTU_FN_NOINLINE void rdoq_sign_hiding(const TuS<Pix> &tu, const uint16_t *blk, double lambda, int qp_scaled, int last_pos, const int16_t *coef, int16_t *q)
 {
-  const int32_t *s_inc = tu.inc(), *s_dec = tu.dec(), *s_sig_inc = tu.sig_inc(), *s_qdelta = tu.qdelta();
-  const int inv_quant = inv_quant_scale(qp_scaled % 6);
-  const long long rd_factor = (long long)(inv_quant * inv_quant * (1 << (2 * (qp_scaled / 6))) / lambda / 16 / (1 << (2 * (PixDepth<Pix>::bd - 8))) + 0.5);
-  const int last_cg = (last_pos - 1) >> 4;
-  for (int cg = last_cg; cg >= 0; --cg) {
-    const uint16_t *pos = blk + (cg << 4);
-    int last_nz = -1, first_nz = 16;
-    for (int k = 15; k >= 0; --k) if (q[pos[k]]) { last_nz = k; break; }
-    for (int k = 0; k <= last_nz; ++k) if (q[pos[k]]) { first_nz = k; break; }
-    if (last_nz - first_nz < 4) continue;
-    const int signbit = q[pos[first_nz]] <= 0;
-    unsigned sum = 0;
-    for (int k = first_nz; k <= last_nz; ++k) sum += (unsigned)(int)q[pos[k]];
-    if (signbit == (int)(sum & 1)) continue;
-    long long best_cost = 0x7FFFFFFFFFFFFFFFLL;
-    int best_pos = 0, best_change = 0;
-    const int start = (cg == last_cg) ? last_nz : 15;
-    for (int k = start; k >= 0; --k) {
-      const int p = pos[k];
-      const long long quant_cost = rd_factor * s_qdelta[p];
-      const int a = iabs((int)q[p]);
-      long long cost;
-      int change;
-      if (a != 0) {
-        long long inc_bits = s_inc[p], dec_bits = s_dec[p];
-        if (a == 1) dec_bits -= CTU_RDOQ_ONE_BIT + s_sig_inc[p];
-        if (cg == last_cg && last_nz == k && a == 1) dec_bits -= 4 * CTU_RDOQ_ONE_BIT;
-        inc_bits = -quant_cost + inc_bits;
-        dec_bits = quant_cost + dec_bits;
-        if (inc_bits < dec_bits) { change = 1; cost = inc_bits; }
-        else {
-          change = -1; cost = dec_bits;
-          if (k == first_nz && a == 1) cost = 0x7FFFFFFFFFFFFFFFLL;
-        }
-      } else {
-        const int bits = CTU_RDOQ_ONE_BIT + s_inc[p] + s_sig_inc[p];
-        const long long aq = quant_cost < 0 ? -quant_cost : quant_cost;
-        cost = -aq + (long long)bits;
-        change = 1;
-        if (k < first_nz && ((coef[p] >= 0) ? 0 : 1) != signbit) cost = 0x7FFFFFFFFFFFFFFFLL;
-      }
-      if (cost < best_cost) { best_cost = cost; best_pos = p; best_change = change; }
-    }
-    if (q[best_pos] == 32767 || q[best_pos] == -32768) best_change = -1;
-    if (coef[best_pos] >= 0) q[best_pos] = (int16_t)(q[best_pos] + best_change);
-    else q[best_pos] = (int16_t)(q[best_pos] - best_change);
-  }
+  kvzcoeff::rdoq_sign_hiding(tu.inc(), tu.dec(), tu.sig_inc(), tu.qdelta(), blk, lambda, PixDepth<Pix>::bd, qp_scaled, last_pos, coef, q);
 }
 
 // RDOQ runs on the first nl = rdoq_lanes() threads of a team (the first warp of a CTA team), whose lanes are `mask`
@@ -819,17 +725,8 @@ CTU_FN_NOINLINE void rdoq_team(const SmTables *T, const SmTables *tb, const CtuC
   for (int i = 0; i < 2 * transform_shift; ++i) err_scale *= 0.5;
   for (int i = 0; i > 2 * transform_shift; --i) err_scale *= 2.0;
   err_scale = err_scale / qc / qc / (1 << (2 * (PixDepth<Pix>::bd - 8)));
-  RdoqModels m;
-  m.eb = tb->ebits;
-  m.sig = cabac + (type ? CTX_SIG_CHROMA : CTX_SIG_LUMA);
-  m.one = cabac + (type ? CTX_ONE_CHROMA : CTX_ONE_LUMA);
-  m.abs = cabac + (type ? CTX_ABS_CHROMA : CTX_ABS_LUMA);
-  m.cg = cabac + CTX_SIG_CG + type;
-  m.last_x = cabac + (type ? CTX_LAST_X_CHROMA : CTX_LAST_X_LUMA);
-  m.last_y = cabac + (type ? CTX_LAST_Y_CHROMA : CTX_LAST_Y_LUMA);
-  m.cbf = cabac + (type ? CTX_CBF_CHROMA : CTX_CBF_LUMA);
-  m.root_cbf = cabac[CTX_ROOT_CBF];
-  auto sig_cost_of = [&](uint8_t code) { return (code >> 6) == 2 ? 0.0 : lambda * rq_ebits(m.sig[code & 63], code >> 6); };
+  const RdoqModels m = rdoq_models(cabac, tb->ebits, type);
+  auto sig_cost_of = [&](uint8_t code) { return (code >> 6) == 2 ? 0.0 : lambda * ebits(m, m.sig[code & 63], code >> 6); };
   auto level0_cost = [&](int blk) { const double e = (double)imin(iabs((int)coef[blk]) * qc, 0x7FFFFFFF - half); return e * e * err_scale; };
   const uint16_t *blk_of = sm_scan(T, scan_idx, log2n - 2);
 
@@ -855,8 +752,8 @@ CTU_FN_NOINLINE void rdoq_team(const SmTables *T, const SmTables *tb, const CtuC
     const int groups = T->group_idx[n - 1];
     for (ctx = 0; ctx < groups; ++ctx) {
       const int o = off + (ctx >> sh);
-      s.last_x_bits[ctx] = bx + rq_ebits(m.last_x[o], 0); bx += rq_ebits(m.last_x[o], 1);
-      s.last_y_bits[ctx] = by + rq_ebits(m.last_y[o], 0); by += rq_ebits(m.last_y[o], 1);
+      s.last_x_bits[ctx] = bx + ebits(m, m.last_x[o], 0); bx += ebits(m, m.last_x[o], 1);
+      s.last_y_bits[ctx] = by + ebits(m, m.last_y[o], 0); by += ebits(m, m.last_y[o], 1);
     }
     s.last_x_bits[ctx] = bx; s.last_y_bits[ctx] = by;
   }
@@ -891,11 +788,11 @@ CTU_FN_NOINLINE void rdoq_team(const SmTables *T, const SmTables *tb, const CtuC
         const bool cand = sp == last_scanpos || ((ld + half) >> q_bits) != 0;
         if (cand) fl |= 2;
         if (sp != last_scanpos) {
-          const int ctx_sig = sig_ctx_inc(T, pattern, scan_idx, blk & (n - 1), blk >> log2n, log2n, type);
-          const double sig0 = lambda * rq_ebits(m.sig[ctx_sig], 0);
+          const int ctx_sig = sig_ctx_inc(T->sig_ctx4, pattern, scan_idx, blk & (n - 1), blk >> log2n, log2n, type);
+          const double sig0 = lambda * ebits(m, m.sig[ctx_sig], 0);
           s.prep_sig0[k] = sig0;
-          s.prep_sig1[k] = lambda * rq_ebits(m.sig[ctx_sig], 1);
-          if (SH) s_sig_inc[blk] = rq_ebits(m.sig[ctx_sig], 1) - rq_ebits(m.sig[ctx_sig], 0);
+          s.prep_sig1[k] = lambda * ebits(m, m.sig[ctx_sig], 1);
+          if (SH) s_sig_inc[blk] = ebits(m, m.sig[ctx_sig], 1) - ebits(m, m.sig[ctx_sig], 0);
           s.prep_ctx_sig[k] = ctx_sig;
           if (!cand) {
             s_sig_code[sp] = (uint8_t)ctx_sig; s_cost_coeff[sp] = c0 + sig0;
@@ -923,7 +820,7 @@ CTU_FN_NOINLINE void rdoq_team(const SmTables *T, const SmTables *tb, const CtuC
           base_cost += c0 + cs;
           st_sig += cs;
           if (k == 0) st_sig0 = cs;
-          if (SH) s_inc[blk_of[sp]] = rq_ebits(m.one[4 * ctx_set + c1], 0);
+          if (SH) s_inc[blk_of[sp]] = ebits(m, m.one[4 * ctx_set + c1], 0);
           if (k == 0 && sp > 0) {
             c2 = 0; rice = 0; c1_idx = 0; c2_idx = 0;
             ctx_set = (sp == 16 || type != 0) ? 0 : 2;
@@ -961,7 +858,7 @@ CTU_FN_NOINLINE void rdoq_team(const SmTables *T, const SmTables *tb, const CtuC
             s_inc[blk] = rdoq_level_rate(m, level + 1, one_ctx, abs_ctx, rice, c1_idx, c2_idx) - now;
             s_dec[blk] = rdoq_level_rate(m, level - 1, one_ctx, abs_ctx, rice, c1_idx, c2_idx) - now;
           } else {
-            s_inc[blk] = rq_ebits(m.one[one_ctx], 0);
+            s_inc[blk] = ebits(m, m.one[one_ctx], 0);
           }
         }
         q[blk] = (int16_t)level;
@@ -992,14 +889,14 @@ CTU_FN_NOINLINE void rdoq_team(const SmTables *T, const SmTables *tb, const CtuC
       if (cg) {
         const int ctx_cg = right || lower;
         if (s_cg_flag[cg_blk] == 0) {
-          s_cg_sig_cost[cg] = lambda * rq_ebits(m.cg[ctx_cg], 0);
+          s_cg_sig_cost[cg] = lambda * ebits(m, m.cg[ctx_cg], 0);
           base_cost += s_cg_sig_cost[cg] - st_sig;
         } else if (cg < cg_last) {
           if (nnz_before_pos0 == 0) { base_cost -= st_sig0; st_sig -= st_sig0; }
           double cost_zero_cg = base_cost;
-          s_cg_sig_cost[cg] = lambda * rq_ebits(m.cg[ctx_cg], 1);
+          s_cg_sig_cost[cg] = lambda * ebits(m, m.cg[ctx_cg], 1);
           base_cost += s_cg_sig_cost[cg];
-          cost_zero_cg += lambda * rq_ebits(m.cg[ctx_cg], 0);
+          cost_zero_cg += lambda * ebits(m, m.cg[ctx_cg], 0);
           cost_zero_cg += st_uncoded;
           cost_zero_cg -= st_coded;
           cost_zero_cg -= st_sig;
@@ -1007,7 +904,7 @@ CTU_FN_NOINLINE void rdoq_team(const SmTables *T, const SmTables *tb, const CtuC
             nz_mask = 0;
             s_cg_flag[cg_blk] = 0;
             base_cost = cost_zero_cg;
-            s_cg_sig_cost[cg] = lambda * rq_ebits(m.cg[ctx_cg], 0);
+            s_cg_sig_cost[cg] = lambda * ebits(m, m.cg[ctx_cg], 0);
             for (int k = 15; k >= 0; --k) {
               const int sp = (cg << 4) + k, blk = blk_of[sp];
               if (q[blk]) { q[blk] = 0; s_cost_coeff[sp] = level0_cost(blk); s_sig_code[sp] = 2 << 6; }
@@ -1027,8 +924,8 @@ CTU_FN_NOINLINE void rdoq_team(const SmTables *T, const SmTables *tb, const CtuC
     double best_cost;
     {
       const int ctx_cbf = type ? tr_depth : !tr_depth;
-      best_cost = block_uncoded_cost + lambda * rq_ebits(m.cbf[ctx_cbf], 0);
-      base_cost += lambda * rq_ebits(m.cbf[ctx_cbf], 1);
+      best_cost = block_uncoded_cost + lambda * ebits(m, m.cbf[ctx_cbf], 0);
+      base_cost += lambda * ebits(m, m.cbf[ctx_cbf], 1);
     }
     int best_last_p1 = 0;
     bool found_last = false;
@@ -1047,8 +944,8 @@ CTU_FN_NOINLINE void rdoq_team(const SmTables *T, const SmTables *tb, const CtuC
         const int py = blk >> log2n, px = blk & (n - 1);
         const int gx = T->group_idx[scan_idx == 2 ? py : px], gy = T->group_idx[scan_idx == 2 ? px : py];
         double bits = s.last_x_bits[gx] + s.last_y_bits[gy];
-        if (gx > 3) bits += CTU_RDOQ_ONE_BIT * ((gx - 2) >> 1);
-        if (gy > 3) bits += CTU_RDOQ_ONE_BIT * ((gy - 2) >> 1);
+        if (gx > 3) bits += RDOQ_ONE_BIT * ((gx - 2) >> 1);
+        if (gy > 3) bits += RDOQ_ONE_BIT * ((gy - 2) >> 1);
         const double total = base_cost + lambda * bits - csk;
         if (total < best_cost) { best_last_p1 = sp + 1; best_cost = total; }
         if (q[blk] > 1) { found_last = true; break; }
@@ -1091,138 +988,32 @@ CTU_FN void cabac_bin(const SmTables *tb, CabacState *c, int off, int val, doubl
   if (c->update) c->ctx[off] = ((st & 1) == val) ? tb->next_mps[st] : tb->next_lps[st];
 }
 
-// the same with an integer accumulator in units of 2^-15 bit
-CTU_FN void cabac_bin_i(const SmTables *tb, CabacState *c, int off, int val, long long *bits)
-{
-  const uint8_t st = c->ctx[off];
-  *bits += tb->ebits[st ^ val];
-  if (c->update) c->ctx[off] = ((st & 1) == val) ? tb->next_mps[st] : tb->next_lps[st];
-}
-
-CTU_FN int coeff_remain_bits(int symbol, int rice)
-{
-  if (symbol < (3 << rice)) return (symbol >> rice) + 1 + rice;
-  int length = rice;
-  symbol -= 3 << rice;
-  while (symbol >= (1 << length)) { symbol -= 1 << length; ++length; }
-  return 3 + length + 1 - rice + length;
-}
-
 // kvz_get_coeff_cost's CABAC branch = kvz_encode_coeff_nxn in counting mode on a copy of the search models that is
 // kept when `update` is set (ref: rdo.c:223-264).  Leader only.  The cost estimate codes tr_skip as 0 (rdo.c:251-258);
-// the tracker of the real coder's models passes the TU's flag.
-#define CTU_NO_MASK 0xFFFFFFFFFFFFFFFFull       // (no unit has all 64 groups... a full 32x32 unit does: then the scan below is harmless)
-CTU_FN_NOINLINE double coeff_cost_serial(const SmTables *T, const SmTables *tb, const CtuConfig *cfg, CabacState *c, const int16_t *coeff, int log2n, int type, int scan_idx, int tr_skip,
-                                         uint64_t known_cg_mask = CTU_NO_MASK)
-{
-  const int n = 1 << log2n, side = n >> 2, ncg = side * side;
-  uint64_t cg_flags = 0;
-  if (known_cg_mask != CTU_NO_MASK) cg_flags = known_cg_mask;
-  else for (int g = 0; g < ncg; ++g) {
-    const int gy = g / side, gx = g - gy * side;
-    bool any = false;
-    for (int r = 0; r < 4 && !any; ++r) {
-      const int16_t *row = coeff + (gy * 4 + r) * n + gx * 4;
-      any = (row[0] | row[1] | row[2] | row[3]) != 0;
-    }
-    if (any) cg_flags |= 1ull << g;
-  }
-  if (!cg_flags) return 0.0;
-  const uint16_t *scan = sm_scan(T, scan_idx, log2n - 2);
-  const uint8_t *scan_cg = T->scan_cg[scan_idx][log2n - 2];
-  int cg_last = ncg - 1;
-  while (!((cg_flags >> scan_cg[cg_last]) & 1)) --cg_last;
-  int scan_last = cg_last * 16 + 15;
-  while (!coeff[scan[scan_last]]) --scan_last;
-  const int pos_last = scan[scan_last];
-
-  // every term is an integer multiple of 2^-15 bit: the reference's double sums are exact, so the integer sum (units of
-  // 2^-15) converted once gives the same double, without a floating-point add chain per bin
-  long long bits = 0;
-  if (n == 4 && cfg->trskip_enable) cabac_bin_i(tb, c, type == 0 ? CTX_TRSKIP_LUMA : CTX_TRSKIP_CHROMA, tr_skip, &bits);
-  long long bits_last = 0;
+// the tracker of the real coder's models passes the TU's flag.  Tables from shared memory (coeff_bits' policy).
+struct CtuCostWalk {
+  const SmTables *T, *tb;
+  const CtuConfig *cfg;
+  CabacState *c;
+  CTU_MFN const uint16_t *scan(int scan_idx, int log2n) const { return sm_scan(T, scan_idx, log2n - 2); }
+  CTU_MFN const uint8_t *scan_cg(int scan_idx, int log2n) const { return T->scan_cg[scan_idx][log2n - 2]; }
+  CTU_MFN int group_idx(int x) const { return T->group_idx[x]; }
+  CTU_MFN const uint8_t *sig_ctx4() const { return T->sig_ctx4; }
+  CTU_MFN int32_t *abs_scratch() const { return tb->abs_scratch[CTU_HALF & 7]; }
+  CTU_MFN bool trskip_enable() const { return cfg->trskip_enable; }
+  CTU_MFN bool signhide() const { return cfg->signhide_enable; }
+  CTU_MFN void bin(int off, int val, long long *bits) const
   {
-    int lx = pos_last & (n - 1), ly = pos_last >> log2n;
-    if (scan_idx == 2) { const int t = lx; lx = ly; ly = t; }
-    const int idx = log2n - 2;
-    const int ctx_offset = type ? 0 : (idx * 3 + (idx + 1) / 4);
-    const int shift = type ? idx : (idx + 3) / 4;
-    const int base_x = type ? CTX_LAST_X_CHROMA : CTX_LAST_X_LUMA;
-    const int base_y = type ? CTX_LAST_Y_CHROMA : CTX_LAST_Y_LUMA;
-    const int gx = T->group_idx[lx], gy = T->group_idx[ly], gmax = T->group_idx[n - 1];
-    for (int k = 0; k < gx; ++k) cabac_bin_i(tb, c, base_x + ctx_offset + (k >> shift), 1, &bits_last);
-    if (gx < gmax) cabac_bin_i(tb, c, base_x + ctx_offset + (gx >> shift), 0, &bits_last);
-    for (int k = 0; k < gy; ++k) cabac_bin_i(tb, c, base_y + ctx_offset + (k >> shift), 1, &bits_last);
-    if (gy < gmax) cabac_bin_i(tb, c, base_y + ctx_offset + (gy >> shift), 0, &bits_last);
-    if (gx > 3) bits_last += (long long)((gx - 2) / 2) << 15;
-    if (gy > 3) bits_last += (long long)((gy - 2) / 2) << 15;
+    const uint8_t st = c->ctx[off];
+    *bits += tb->ebits[st ^ val];
+    if (c->update) c->ctx[off] = ((st & 1) == val) ? tb->next_mps[st] : tb->next_lps[st];
   }
-  const int base_cg = CTX_SIG_CG + type;
-  const int base_sig = type == 0 ? CTX_SIG_LUMA : CTX_SIG_CHROMA;
-  int c1 = 1;
-  int scan_pos_sig = scan_last;
-  for (int i = cg_last; i >= 0; --i) {
-    const int sub_pos = i << 4;
-    int32_t *abs_coeff = tb->abs_scratch[CTU_HALF & 7];
-    const int cg_blk = scan_cg[i];
-    const int cgy = cg_blk / side, cgx = cg_blk - cgy * side;
-    int last_nz = -1, first_nz = 16, num_nz = 0, rice = 0;
-    if (scan_pos_sig == scan_last) {
-      abs_coeff[0] = iabs((int)coeff[pos_last]);
-      num_nz = 1; last_nz = scan_pos_sig; first_nz = scan_pos_sig;
-      --scan_pos_sig;
-    }
-    const int right = (cgx < side - 1) ? (int)((cg_flags >> (cgy * side + cgx + 1)) & 1) : 0;
-    const int lower = (cgy < side - 1) ? (int)((cg_flags >> ((cgy + 1) * side + cgx)) & 1) : 0;
-    if (i == cg_last || i == 0) cg_flags |= 1ull << cg_blk;
-    else cabac_bin_i(tb, c, base_cg + (right || lower), (int)((cg_flags >> cg_blk) & 1), &bits);
-    if ((cg_flags >> cg_blk) & 1) {
-      const int pattern = (n == 4) ? -1 : right + (lower << 1);
-      for (; scan_pos_sig >= sub_pos; --scan_pos_sig) {
-        const int blk = scan[scan_pos_sig];
-        const int sig = coeff[blk] != 0;
-        if (scan_pos_sig > sub_pos || i == 0 || num_nz)
-          cabac_bin_i(tb, c, base_sig + sig_ctx_inc(T, pattern, scan_idx, blk & (n - 1), blk >> log2n, log2n, type), sig, &bits);
-        if (sig) {
-          abs_coeff[num_nz++] = iabs((int)coeff[blk]);
-          if (last_nz == -1) last_nz = scan_pos_sig;
-          first_nz = scan_pos_sig;
-        }
-      }
-    } else {
-      scan_pos_sig = sub_pos - 1;
-    }
-    if (num_nz > 0) {
-      const bool sign_hidden = last_nz - first_nz >= 4;
-      int ctx_set = (i > 0 && type == 0) ? 2 : 0;
-      if (c1 == 0) ++ctx_set;
-      c1 = 1;
-      const int base_one = (type == 0 ? CTX_ONE_LUMA : CTX_ONE_CHROMA) + 4 * ctx_set;
-      const int num_c1 = imin(num_nz, 8);
-      int first_c2 = -1;
-      for (int k = 0; k < num_c1; ++k) {
-        const int symbol = abs_coeff[k] > 1;
-        cabac_bin_i(tb, c, base_one + c1, symbol, &bits);
-        if (symbol) { c1 = 0; if (first_c2 == -1) first_c2 = k; }
-        else if (c1 < 3 && c1 > 0) ++c1;
-      }
-      if (c1 == 0 && first_c2 != -1)
-        cabac_bin_i(tb, c, (type == 0 ? CTX_ABS_LUMA : CTX_ABS_CHROMA) + ctx_set, abs_coeff[first_c2] > 2, &bits);
-      bits += (long long)((cfg->signhide_enable && sign_hidden) ? num_nz - 1 : num_nz) << 15;
-      if (c1 == 0 || num_nz > 8) {
-        int first_coeff2 = 1;
-        for (int k = 0; k < num_nz; ++k) {
-          const int base_level = (k < 8) ? (2 + first_coeff2) : 1;
-          if (abs_coeff[k] >= base_level) {
-            bits += (long long)coeff_remain_bits(abs_coeff[k] - base_level, rice) << 15;
-            if (abs_coeff[k] > 3 * (1 << rice)) rice = imin(rice + 1, 4);
-          }
-          if (abs_coeff[k] >= 2) first_coeff2 = 0;
-        }
-      }
-    }
-  }
-  return (double)(bits_last + bits) * (1.0 / 32768.0);
+};
+CTU_FN_NOINLINE double coeff_cost_serial(const SmTables *T, const SmTables *tb, const CtuConfig *cfg, CabacState *c, const int16_t *coeff, int log2n, int type, int scan_idx, int tr_skip,
+                                         uint64_t known_cg_mask = COEFF_NO_MASK)
+{
+  CtuCostWalk w = { T, tb, cfg, c };
+  return (double)coeff_bits(w, coeff, log2n, type, scan_idx, tr_skip, known_cg_mask) * (1.0 / 32768.0);
 }
 
 // ------------------------------------------------------------------------------------------------ one transform unit

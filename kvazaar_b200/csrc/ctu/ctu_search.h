@@ -205,7 +205,7 @@ CTU_FN int stage_key_of(int xl, int yl, int depth) { return (xl << 16) | (yl << 
 // coefficients of the unit of `color` at (xl, yl, depth) on level L: the staged copy when it is this unit's
 template <typename Pix> CTU_FN const int16_t *unit_coeffs(const CtxT<Pix> &c, LcuLevel<Pix> *L, int color, int xl, int yl, int depth, uint64_t *mask)
 {
-  *mask = CTU_NO_MASK;
+  *mask = COEFF_NO_MASK;
   if (c.S->stage_key[color] == stage_key_of(xl, yl, depth)) { *mask = c.S->stage_mask[color]; return color == 0 ? c.S->stage_y : c.S->stage_c[color - 1]; }
   if (color == 0) return &L->coeff_y[zorder(64, xl, yl)];
   return (color == 1 ? L->coeff_u : L->coeff_v) + zorder(32, xl >> 1, yl >> 1);

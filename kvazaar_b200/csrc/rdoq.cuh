@@ -15,18 +15,7 @@
 
 namespace kvzc {
 
-// HM's fractional-bit estimates per CABAC state (15 fractional bits), split by symbol = MPS / LPS
-// (kvz_entropy_bits, rdo.c:69-79: entry [2s] is the MPS cost of state s, [2s + 1] the LPS cost)
-static __device__ const int32_t c_ebits_mps[64] = {
-  32768, 30426, 28306, 26378, 24617, 23005, 21523, 20159, 18899, 17734, 16653, 15650, 14717, 13849, 13038, 12282,
-  11575, 10914, 10294, 9714, 9169, 8658, 8178, 7727, 7303, 6903, 6527, 6173, 5840, 5525, 5228, 4948,
-  4684, 4435, 4199, 3977, 3767, 3568, 3380, 3202, 3034, 2876, 2725, 2583, 2448, 2321, 2200, 2086,
-  1978, 1875, 1778, 1686, 1599, 1517, 1439, 1364, 1294, 1228, 1165, 1105, 1048, 994, 943, 895 };
-static __device__ const int32_t c_ebits_lps[64] = {
-  32768, 35232, 37696, 40159, 42623, 45087, 47551, 50015, 52479, 54942, 57406, 59870, 62334, 64798, 67262, 69725,
-  72189, 74653, 77117, 79581, 82044, 84508, 86972, 89436, 91900, 94363, 96827, 99291, 101755, 104219, 106683, 109146,
-  111610, 114074, 116538, 119002, 121465, 123929, 126393, 128857, 131321, 133785, 136248, 138712, 141176, 143640, 146104, 148568,
-  151031, 153495, 155959, 158423, 160887, 163351, 165814, 168278, 170742, 173207, 175669, 178134, 180598, 183061, 185525, 187989 };
+static __device__ const int32_t c_ebits_mps[64] = { COEFF_EBITS_MPS }, c_ebits_lps[64] = { COEFF_EBITS_LPS };
 
 // The 128-entry table in the reference's indexing (state byte ^ bin), staged in shared memory by the kernels: lanes
 // look up different states at the same time, which constant memory would serialise.
@@ -35,17 +24,11 @@ __device__ __forceinline__ void rdoq_load_ebits(int32_t *table /* [128] */)
   for (int i = threadIdx.x; i < 128; i += blockDim.x) table[i] = (i & 1) ? c_ebits_lps[i >> 1] : c_ebits_mps[i >> 1];
 }
 
-constexpr int RDOQ_ONE_BIT = 1 << 15;
-
-// position group of a last-significant coordinate (g_group_idx, rdo.c: 0,1,2,3,4,4,5,5,6,6,6,6,7,7,7,7,8..,9..)
-__device__ __forceinline__ int last_group(int x) { if (x < 4) return x; const int l = 31 - __clz(x); return 2 * l + ((x >> (l - 1)) & 1); }
-
 // scan position -> raster position of the 32x32 diagonal scan, shared by every 32x32 TU (filled once per process by
 // rdoq_init_tables); smaller blocks build their table in shared memory
 static __device__ uint16_t g_scan_diag32[1024];
 static __global__ void rdoq_init_scan32_kernel() { g_scan_diag32[threadIdx.x] = (uint16_t)scan_pos(0, 5, threadIdx.x); }
 
-// SH = sign hiding enabled: only then the per-position rate tables of kvz_sh_rates_t exist
 // SH = sign hiding enabled: only then the per-position rate tables of kvz_sh_rates_t exist.
 // cost_sig (rdo.c:683) is kept as one byte per position: the significance context (6 bits) and which of its two bin
 // costs the position carries (0: flag = 0, 1: flag = 1, 2: none -- the last coefficient or a zeroed group); the double
@@ -66,150 +49,6 @@ struct RdoqScratch {
   int32_t prep_ld[16], prep_ctx_sig[16];
   int32_t best_last_p1;
 };
-
-struct RdoqModels {      // views into the kvz_cuda_cabac_ctx image for one texture type
-  const uint8_t *sig, *one, *abs, *cg, *last_x, *last_y, *cbf;
-  const int32_t *eb;     // entropy-bit table, see rdoq_load_ebits
-  uint8_t root_cbf;
-};
-// cost in 1/32768 bits of coding `bin` with the context whose state byte is `st` (bit 0 = MPS value)
-#define ebits(st, bin) (m.eb[(st) ^ (bin)])
-
-__device__ __forceinline__ RdoqModels rdoq_models(const kvz_cuda_cabac_ctx *c, const int32_t *eb, int type)
-{
-  RdoqModels m;
-  m.eb = eb;
-  m.sig = type ? c->cu_sig_model_chroma : c->cu_sig_model_luma;
-  m.one = type ? c->cu_one_model_chroma : c->cu_one_model_luma;
-  m.abs = type ? c->cu_abs_model_chroma : c->cu_abs_model_luma;
-  m.cg = c->cu_sig_coeff_group_model + type;               // rdo.c:720: indexed by type (0 luma, 2 chroma)
-  m.last_x = type ? c->cu_ctx_last_x_chroma : c->cu_ctx_last_x_luma;
-  m.last_y = type ? c->cu_ctx_last_y_chroma : c->cu_ctx_last_y_luma;
-  m.cbf = type ? c->qt_cbf_model_chroma : c->qt_cbf_model_luma;
-  m.root_cbf = c->cu_qt_root_cbf_model;
-  return m;
-}
-
-// rate of the level bins of |level| given the greater1 / greater2 contexts and the Rice parameter (rdo.c:346-393)
-__device__ __forceinline__ int rdoq_level_rate(const RdoqModels &m, uint32_t abs_level, int ctx_one, int ctx_abs, int rice, uint32_t c1_idx, uint32_t c2_idx)
-{
-  int rate = RDOQ_ONE_BIT;                                               // the sign bin
-  const uint32_t base_level = (c1_idx < 8) ? (2 + (c2_idx < 1)) : 1;
-  if (abs_level >= base_level) {
-    int symbol = (int)(abs_level - base_level);
-    if (symbol < (3 << rice)) {
-      rate += ((symbol >> rice) + 1 + rice) * RDOQ_ONE_BIT;
-    } else {
-      int length = rice;
-      symbol -= 3 << rice;
-      while (symbol >= (1 << length)) symbol -= 1 << (length++);
-      rate += (3 + length + 1 - rice + length) * RDOQ_ONE_BIT;
-    }
-    if (c1_idx < 8) {
-      rate += ebits(m.one[ctx_one], 1);
-      if (c2_idx < 1) rate += ebits(m.abs[ctx_abs], 1);
-    }
-  } else if (abs_level == 1) {
-    rate += ebits(m.one[ctx_one], 0);
-  } else if (abs_level == 2) {
-    rate += ebits(m.one[ctx_one], 1);
-    rate += ebits(m.abs[ctx_abs], 0);
-  }
-  return rate;
-}
-
-// best level of one coefficient (rdo.c:413-452); cost0 = distortion of level 0
-__device__ __forceinline__ uint32_t rdoq_pick_level(const RdoqModels &m, double lambda, double &cost, double cost0, double &cost_sig, int level_double,
-                                                    uint32_t max_abs_level, int ctx_sig, int ctx_one, int ctx_abs, int rice, uint32_t c1_idx,
-                                                    uint32_t c2_idx, int q_bits, double err_scale, bool last)
-{
-  double sig_cost_now = 0;
-  uint32_t best = 0;
-  if (!last && max_abs_level < 3) {
-    cost_sig = lambda * ebits(m.sig[ctx_sig], 0);
-    cost = cost0 + cost_sig;
-    if (max_abs_level == 0) return 0;
-  } else {
-    cost = 1.7e+308;
-  }
-  if (!last) sig_cost_now = lambda * ebits(m.sig[ctx_sig], 1);
-  const int lo = max_abs_level > 1 ? (int)max_abs_level - 1 : 1;
-  for (int lvl = (int)max_abs_level; lvl >= lo; --lvl) {
-    const double err = (double)(level_double - lvl * (1 << q_bits));
-    double c = err * err * err_scale + lambda * rdoq_level_rate(m, (uint32_t)lvl, ctx_one, ctx_abs, rice, c1_idx, c2_idx);
-    c += sig_cost_now;
-    if (c < cost) { best = (uint32_t)lvl; cost = c; cost_sig = sig_cost_now; }
-  }
-  return best;
-}
-
-// context increment of sig_coeff_flag (context.c:366-397)
-__device__ __forceinline__ int rdoq_sig_ctx(int pattern, int scan_idx, int px, int py, int log2n, int type)
-{
-  if (px + py == 0) return 0;
-  if (log2n == 2) { const int map[16] = { 0, 1, 4, 5, 2, 3, 4, 5, 6, 6, 8, 8, 7, 7, 8, 8 }; return map[4 * py + px]; }
-  const int offset = (log2n == 3) ? (scan_idx == 0 ? 9 : 15) : (type == 0 ? 21 : 12);
-  const int sx = px & 3, sy = py & 3;
-  int cnt;
-  if (pattern == 0) cnt = (sx + sy <= 2) ? ((sx + sy == 0) ? 2 : 1) : 0;
-  else if (pattern == 1) cnt = (sy <= 1) ? ((sy == 0) ? 2 : 1) : 0;
-  else if (pattern == 2) cnt = (sx <= 1) ? ((sx == 0) ? 2 : 1) : 0;
-  else cnt = 2;
-  return ((type == 0 && ((px >> 2) + (py >> 2)) > 0) ? 3 : 0) + offset + cnt;
-}
-
-// Sign-bit hiding on RDOQ output (rdo.c:518-653).  Serial; one thread.
-template <class Scratch, class BlkT>
-__device__ void rdoq_sign_hiding(const Scratch &s, const BlkT *blk, double lambda, int bitdepth, int qp_scaled, int scan_idx, int log2n, int last_pos,
-                                 const int16_t *coef, int16_t *q)
-{
-  const int inv_quant = c_inv_quant_scales[qp_scaled % 6];
-  const long long rd_factor = (long long)(inv_quant * inv_quant * (1 << (2 * (qp_scaled / 6))) / lambda / 16 / (1 << (2 * (bitdepth - 8))) + 0.5);
-  const int last_cg = (last_pos - 1) >> 4;
-  for (int cg = last_cg; cg >= 0; --cg) {
-    const int base = cg << 4;
-    const BlkT *pos = blk + base;
-    int last_nz = -1, first_nz = 16;
-    for (int k = 15; k >= 0; --k) if (q[pos[k]]) { last_nz = k; break; }
-    for (int k = 0; k <= last_nz; ++k) if (q[pos[k]]) { first_nz = k; break; }
-    if (last_nz - first_nz < 4) continue;
-    const int signbit = q[pos[first_nz]] <= 0;
-    unsigned sum = 0;
-    for (int k = first_nz; k <= last_nz; ++k) sum += (unsigned)(int)q[pos[k]];
-    if (signbit == (int)(sum & 1)) continue;
-    long long best_cost = 0x7FFFFFFFFFFFFFFFLL;
-    int best_pos = 0, best_change = 0;
-    const int start = (cg == last_cg) ? last_nz : 15;
-    for (int k = start; k >= 0; --k) {
-      const int p = pos[k];
-      const long long quant_cost = rd_factor * s.qdelta[p];
-      const int a = abs((int)q[p]);
-      long long cost;
-      int change;
-      if (a != 0) {
-        long long inc_bits = s.inc[p], dec_bits = s.dec[p];
-        if (a == 1) dec_bits -= RDOQ_ONE_BIT + s.sig_inc[p];
-        if (cg == last_cg && last_nz == k && a == 1) dec_bits -= 4 * RDOQ_ONE_BIT;
-        inc_bits = -quant_cost + inc_bits * 1;            // PRECISION_INC = 15 - CTX_FRAC_BITS = 0
-        dec_bits = quant_cost + dec_bits * 1;
-        if (inc_bits < dec_bits) { change = 1; cost = inc_bits; }
-        else {
-          change = -1; cost = dec_bits;
-          if (k == first_nz && a == 1) cost = 0x7FFFFFFFFFFFFFFFLL;
-        }
-      } else {
-        const int bits = RDOQ_ONE_BIT + s.inc[p] + s.sig_inc[p];
-        cost = -llabs(quant_cost) + (long long)bits;
-        change = 1;
-        if (k < first_nz && ((coef[p] >= 0) ? 0 : 1) != signbit) cost = 0x7FFFFFFFFFFFFFFFLL;
-      }
-      if (cost < best_cost) { best_cost = cost; best_pos = p; best_change = change; }
-    }
-    if (q[best_pos] == 32767 || q[best_pos] == -32768) best_change = -1;
-    if (coef[best_pos] >= 0) q[best_pos] = (int16_t)(q[best_pos] + best_change);
-    else q[best_pos] = (int16_t)(q[best_pos] - best_change);
-  }
-}
 
 // kvz_rdoq for one TU by one warp (all 32 lanes must call; `lane` = lane id).  coef / q: n x n row-major in shared
 // memory.  type: 0 luma, 2 chroma (the reference passes 2 for U and V, quant-generic.c:239).  block_type: 1 intra,
@@ -235,7 +74,7 @@ __device__ void rdoq_tu(const kvz_cuda_rdoq_params &p, const kvz_cuda_cabac_ctx 
   const RdoqModels m = rdoq_models(cabac, ebits_table, type);
   // distortion of quantising the coefficient at raster position blk to 0 (cost_coeff0, rdo.c:770-771)
   // cost_sig of a position from its code byte
-  auto sig_cost_of = [&](uint8_t code) { return (code >> 6) == 2 ? 0.0 : lambda * ebits(m.sig[code & 63], code >> 6); };
+  auto sig_cost_of = [&](uint8_t code) { return (code >> 6) == 2 ? 0.0 : lambda * ebits(m, m.sig[code & 63], code >> 6); };
   auto level0_cost = [&](int blk) { const double e = (double)min(abs((int)coef[blk]) * qc, 0x7FFFFFFF - half); return e * e * err_scale; };
 
   // ---- scan table and last significant scan position (find_last_scanpos)
@@ -266,8 +105,8 @@ __device__ void rdoq_tu(const kvz_cuda_rdoq_params &p, const kvz_cuda_cabac_ctx 
     const int groups = last_group(n - 1);
     for (ctx = 0; ctx < groups; ++ctx) {
       const int o = off + (ctx >> sh);
-      s.last_x_bits[ctx] = bx + ebits(m.last_x[o], 0); bx += ebits(m.last_x[o], 1);
-      s.last_y_bits[ctx] = by + ebits(m.last_y[o], 0); by += ebits(m.last_y[o], 1);
+      s.last_x_bits[ctx] = bx + ebits(m, m.last_x[o], 0); bx += ebits(m, m.last_x[o], 1);
+      s.last_y_bits[ctx] = by + ebits(m, m.last_y[o], 0); by += ebits(m, m.last_y[o], 1);
     }
     s.last_x_bits[ctx] = bx; s.last_y_bits[ctx] = by;
   }
@@ -304,11 +143,11 @@ __device__ void rdoq_tu(const kvz_cuda_rdoq_params &p, const kvz_cuda_cabac_ctx 
         s.prep_c0[lane] = c0;
         cand = sp == last_scanpos || ((ld + half) >> q_bits) != 0;
         if (sp != last_scanpos) {
-          const int ctx_sig = rdoq_sig_ctx(pattern, scan_idx, blk & (n - 1), blk >> log2n, log2n, type);
-          const double sig0 = lambda * ebits(m.sig[ctx_sig], 0);
+          const int ctx_sig = sig_ctx_inc(SigCtx4(), pattern, scan_idx, blk & (n - 1), blk >> log2n, log2n, type);
+          const double sig0 = lambda * ebits(m, m.sig[ctx_sig], 0);
           s.prep_sig0[lane] = sig0;
-          s.prep_sig1[lane] = lambda * ebits(m.sig[ctx_sig], 1);
-          if (SH) s.sig_inc[blk] = ebits(m.sig[ctx_sig], 1) - ebits(m.sig[ctx_sig], 0);
+          s.prep_sig1[lane] = lambda * ebits(m, m.sig[ctx_sig], 1);
+          if (SH) s.sig_inc[blk] = ebits(m, m.sig[ctx_sig], 1) - ebits(m, m.sig[ctx_sig], 0);
           s.prep_ctx_sig[lane] = ctx_sig;
           if (!cand) {
             s.sig_code[sp] = (uint8_t)ctx_sig; s.cost_coeff[sp] = c0 + sig0;
@@ -347,7 +186,7 @@ __device__ void rdoq_tu(const kvz_cuda_rdoq_params &p, const kvz_cuda_cabac_ctx 
           base_cost += c0 + cs;
           st_sig += cs;
           if (k == 0) st_sig0 = cs;
-          if (SH) s.inc[blk_of[sp]] = ebits(m.one[4 * ctx_set + c1], 0);
+          if (SH) s.inc[blk_of[sp]] = ebits(m, m.one[4 * ctx_set + c1], 0);
           if (k == 0 && sp > 0) {
             c2 = 0; rice = 0; c1_idx = 0; c2_idx = 0;
             ctx_set = (sp == 16 || type != 0) ? 0 : 2;
@@ -386,7 +225,7 @@ __device__ void rdoq_tu(const kvz_cuda_rdoq_params &p, const kvz_cuda_cabac_ctx 
             s.inc[blk] = rdoq_level_rate(m, level + 1, one_ctx, abs_ctx, rice, c1_idx, c2_idx) - now;
             s.dec[blk] = rdoq_level_rate(m, level - 1, one_ctx, abs_ctx, rice, c1_idx, c2_idx) - now;
           } else {
-            s.inc[blk] = ebits(m.one[one_ctx], 0);
+            s.inc[blk] = ebits(m, m.one[one_ctx], 0);
           }
         }
         q[blk] = (int16_t)level;
@@ -417,14 +256,14 @@ __device__ void rdoq_tu(const kvz_cuda_rdoq_params &p, const kvz_cuda_cabac_ctx 
       if (cg) {
         const int ctx_cg = right || lower;
         if (s.cg_flag[cg_blk] == 0) {
-          s.cg_sig_cost[cg] = lambda * ebits(m.cg[ctx_cg], 0);
+          s.cg_sig_cost[cg] = lambda * ebits(m, m.cg[ctx_cg], 0);
           base_cost += s.cg_sig_cost[cg] - st_sig;
         } else if (cg < cg_last) {
           if (nnz_before_pos0 == 0) { base_cost -= st_sig0; st_sig -= st_sig0; }
           double cost_zero_cg = base_cost;
-          s.cg_sig_cost[cg] = lambda * ebits(m.cg[ctx_cg], 1);
+          s.cg_sig_cost[cg] = lambda * ebits(m, m.cg[ctx_cg], 1);
           base_cost += s.cg_sig_cost[cg];
-          cost_zero_cg += lambda * ebits(m.cg[ctx_cg], 0);
+          cost_zero_cg += lambda * ebits(m, m.cg[ctx_cg], 0);
           cost_zero_cg += st_uncoded;
           cost_zero_cg -= st_coded;
           cost_zero_cg -= st_sig;
@@ -432,7 +271,7 @@ __device__ void rdoq_tu(const kvz_cuda_rdoq_params &p, const kvz_cuda_cabac_ctx 
             nz_mask = 0;
             s.cg_flag[cg_blk] = 0;
             base_cost = cost_zero_cg;
-            s.cg_sig_cost[cg] = lambda * ebits(m.cg[ctx_cg], 0);
+            s.cg_sig_cost[cg] = lambda * ebits(m, m.cg[ctx_cg], 0);
             for (int k = 15; k >= 0; --k) {
               const int sp = (cg << 4) + k, blk = blk_of[sp];
               if (q[blk]) { q[blk] = 0; s.cost_coeff[sp] = level0_cost(blk); s.sig_code[sp] = 2 << 6; }
@@ -451,12 +290,12 @@ __device__ void rdoq_tu(const kvz_cuda_rdoq_params &p, const kvz_cuda_cabac_ctx 
     // ---- best last position (rdo.c:884-945)
     double best_cost;
     if (block_type != 1 && type == 0) {
-      best_cost = block_uncoded_cost + lambda * ebits(m.root_cbf, 0);
-      base_cost += lambda * ebits(m.root_cbf, 1);
+      best_cost = block_uncoded_cost + lambda * ebits(m, m.root_cbf, 0);
+      base_cost += lambda * ebits(m, m.root_cbf, 1);
     } else {
       const int ctx_cbf = type ? tr_depth : !tr_depth;
-      best_cost = block_uncoded_cost + lambda * ebits(m.cbf[ctx_cbf], 0);
-      base_cost += lambda * ebits(m.cbf[ctx_cbf], 1);
+      best_cost = block_uncoded_cost + lambda * ebits(m, m.cbf[ctx_cbf], 0);
+      base_cost += lambda * ebits(m, m.cbf[ctx_cbf], 1);
     }
     int best_last_p1 = 0;
     bool found_last = false;
@@ -513,7 +352,7 @@ __device__ void rdoq_tu(const kvz_cuda_rdoq_params &p, const kvz_cuda_cabac_ctx 
   if constexpr (SH) {
     abs_sum = warp_sum(abs_sum);
     __syncwarp();
-    if (lane == 0 && abs_sum >= 2) rdoq_sign_hiding(s, blk_of, lambda, p.bitdepth, qp_scaled, scan_idx, log2n, best_last_p1, coef, q);
+    if (lane == 0 && abs_sum >= 2) rdoq_sign_hiding(s.inc, s.dec, s.sig_inc, s.qdelta, blk_of, lambda, p.bitdepth, qp_scaled, best_last_p1, coef, q);
   }
   __syncwarp();
 }
@@ -565,8 +404,8 @@ __device__ void rdoq_tu_thread(const kvz_cuda_rdoq_params &p, const kvz_cuda_cab
     const int groups = last_group(n - 1);
     for (ctx = 0; ctx < groups; ++ctx) {
       const int o = off + (ctx >> sh);
-      s.last_x_bits[ctx] = bx + ebits(m.last_x[o], 0); bx += ebits(m.last_x[o], 1);
-      s.last_y_bits[ctx] = by + ebits(m.last_y[o], 0); by += ebits(m.last_y[o], 1);
+      s.last_x_bits[ctx] = bx + ebits(m, m.last_x[o], 0); bx += ebits(m, m.last_x[o], 1);
+      s.last_y_bits[ctx] = by + ebits(m, m.last_y[o], 0); by += ebits(m, m.last_y[o], 1);
     }
     s.last_x_bits[ctx] = bx; s.last_y_bits[ctx] = by;
   }
@@ -600,15 +439,15 @@ __device__ void rdoq_tu_thread(const kvz_cuda_rdoq_params &p, const kvz_cuda_cab
       const bool last = sp == last_scanpos;
       int ctx_sig = 0;
       if (!last) {
-        ctx_sig = rdoq_sig_ctx(pattern, scan_idx, blk & (n - 1), blk >> log2n, log2n, type);
-        if (SH) s.sig_inc[blk] = ebits(m.sig[ctx_sig], 1) - ebits(m.sig[ctx_sig], 0);
+        ctx_sig = sig_ctx_inc(SigCtx4(), pattern, scan_idx, blk & (n - 1), blk >> log2n, log2n, type);
+        if (SH) s.sig_inc[blk] = ebits(m, m.sig[ctx_sig], 1) - ebits(m, m.sig[ctx_sig], 0);
       }
       uint32_t level = 0;
       double cc, cs = 0;
-      if (!last && max_abs < 3) { cs = lambda * ebits(m.sig[ctx_sig], 0); cc = c0 + cs; }
+      if (!last && max_abs < 3) { cs = lambda * ebits(m, m.sig[ctx_sig], 0); cc = c0 + cs; }
       else cc = 1.7e+308;
       if (max_abs != 0) {
-        const double sig_now = last ? 0.0 : lambda * ebits(m.sig[ctx_sig], 1);
+        const double sig_now = last ? 0.0 : lambda * ebits(m, m.sig[ctx_sig], 1);
         const int lo = max_abs > 1 ? (int)max_abs - 1 : 1;
         for (int lvl = (int)max_abs; lvl >= lo; --lvl) {
           const double err = (double)(ld - lvl * (1 << q_bits));
@@ -626,7 +465,7 @@ __device__ void rdoq_tu_thread(const kvz_cuda_rdoq_params &p, const kvz_cuda_cab
           s.inc[blk] = rdoq_level_rate(m, level + 1, one_ctx, abs_ctx, rice, c1_idx, c2_idx) - now;
           s.dec[blk] = rdoq_level_rate(m, level - 1, one_ctx, abs_ctx, rice, c1_idx, c2_idx) - now;
         } else {
-          s.inc[blk] = ebits(m.one[one_ctx], 0);
+          s.inc[blk] = ebits(m, m.one[one_ctx], 0);
         }
       }
       q[blk] = (int16_t)level;
@@ -654,21 +493,21 @@ __device__ void rdoq_tu_thread(const kvz_cuda_rdoq_params &p, const kvz_cuda_cab
     if (cg) {
       const int ctx_cg = right || lower;
       if (s.cg_flag[cg_blk] == 0) {
-        s.cg_sig_cost[cg] = lambda * ebits(m.cg[ctx_cg], 0);
+        s.cg_sig_cost[cg] = lambda * ebits(m, m.cg[ctx_cg], 0);
         base_cost += s.cg_sig_cost[cg] - st_sig;
       } else if (cg < cg_last) {
         if (nnz_before_pos0 == 0) { base_cost -= st_sig0; st_sig -= st_sig0; }
         double cost_zero_cg = base_cost;
-        s.cg_sig_cost[cg] = lambda * ebits(m.cg[ctx_cg], 1);
+        s.cg_sig_cost[cg] = lambda * ebits(m, m.cg[ctx_cg], 1);
         base_cost += s.cg_sig_cost[cg];
-        cost_zero_cg += lambda * ebits(m.cg[ctx_cg], 0);
+        cost_zero_cg += lambda * ebits(m, m.cg[ctx_cg], 0);
         cost_zero_cg += st_uncoded;
         cost_zero_cg -= st_coded;
         cost_zero_cg -= st_sig;
         if (cost_zero_cg < base_cost) {
           s.cg_flag[cg_blk] = 0;
           base_cost = cost_zero_cg;
-          s.cg_sig_cost[cg] = lambda * ebits(m.cg[ctx_cg], 0);
+          s.cg_sig_cost[cg] = lambda * ebits(m, m.cg[ctx_cg], 0);
           for (int k = 15; k >= 0; --k) {
             const int sp = (cg << 4) + k, blk = s.blk[sp];
             if (q[blk]) { q[blk] = 0; const double e = (double)level_double(blk); s.cost_coeff[sp] = e * e * err_scale; s.cost_sig[sp] = 0; }
@@ -683,12 +522,12 @@ __device__ void rdoq_tu_thread(const kvz_cuda_rdoq_params &p, const kvz_cuda_cab
   // best last position (rdo.c:884-945)
   double best_cost;
   if (block_type != 1 && type == 0) {
-    best_cost = block_uncoded_cost + lambda * ebits(m.root_cbf, 0);
-    base_cost += lambda * ebits(m.root_cbf, 1);
+    best_cost = block_uncoded_cost + lambda * ebits(m, m.root_cbf, 0);
+    base_cost += lambda * ebits(m, m.root_cbf, 1);
   } else {
     const int ctx_cbf = type ? tr_depth : !tr_depth;
-    best_cost = block_uncoded_cost + lambda * ebits(m.cbf[ctx_cbf], 0);
-    base_cost += lambda * ebits(m.cbf[ctx_cbf], 1);
+    best_cost = block_uncoded_cost + lambda * ebits(m, m.cbf[ctx_cbf], 0);
+    base_cost += lambda * ebits(m, m.cbf[ctx_cbf], 1);
   }
   int best_last_p1 = 0;
   bool found_last = false;
@@ -727,7 +566,7 @@ __device__ void rdoq_tu_thread(const kvz_cuda_rdoq_params &p, const kvz_cuda_cab
   }
   for (int sp = best_last_p1; sp <= last_scanpos; ++sp) q[s.blk[sp]] = 0;
   if constexpr (SH) {
-    if (abs_sum >= 2) rdoq_sign_hiding(s, s.blk, lambda, p.bitdepth, qp_scaled, scan_idx, log2n, best_last_p1, coef, q);
+    if (abs_sum >= 2) rdoq_sign_hiding(s.inc, s.dec, s.sig_inc, s.qdelta, s.blk, lambda, p.bitdepth, qp_scaled, best_last_p1, coef, q);
   }
 }
 

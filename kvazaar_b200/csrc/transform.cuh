@@ -6,8 +6,11 @@
 // Integer addition is associative, so a plain dot product reproduces them bit for bit.
 #pragma once
 #include "common.cuh"
+#include "coeff_rules.h"
 
 namespace kvzc {
+
+using namespace kvzcoeff;
 
 // C[m], m = 0..32: the HEVC core-transform coefficient list; M32[k][i] = sgn * C[fold((k*(2i+1)) mod 128)]
 // (cosine symmetries C[64-m] = -C[m], C[128-m] = C[m]); the N-point matrix takes rows 0, 32/N, 2*32/N, ...
@@ -123,43 +126,17 @@ __device__ __forceinline__ void mat_pass_dp2a(const int16_t *src, int16_t *out, 
 __device__ __forceinline__ int ilog2(int n) { return 31 - __clz(n); }
 
 // ---- quantisation ---------------------------------------------------------------------------
-static __constant__ int c_quant_scales[6] = { 26214, 23302, 20560, 18396, 16384, 14564 };   // ref: scalinglist.c:78
-static __constant__ int c_inv_quant_scales[6] = { 40, 45, 51, 57, 64, 72 };                 // ref: scalinglist.c:79
-
-// ref: transform.c:56-62,88-102 (kvz_get_scaled_qp with the chroma QP mapping table folded into its rule)
-__device__ __host__ __forceinline__ int scaled_qp(int type, int qp, int qp_offset)
-{
-  if (type == 0) return qp + qp_offset;
-  int q = qp < -qp_offset ? -qp_offset : (qp > 57 ? 57 : qp);
-  if (q < 0) return q + qp_offset;
-  int c;
-  if (q < 30) c = q;
-  else if (q >= 44) c = q - 6;
-  else { const int mid[14] = { 29, 30, 31, 32, 33, 33, 34, 34, 35, 35, 36, 36, 37, 37 }; c = mid[q - 30]; }
-  return c + qp_offset;
-}
+static __constant__ int c_quant_scales[6] = { COEFF_QUANT_SCALES };
+static __constant__ int c_inv_quant_scales[6] = { COEFF_INV_QUANT_SCALES };
 
 // position of scan index `idx` for an n x n block (ref: tables.c kvz_g_sig_last_scan): 4x4 coefficient groups
-// visited in scan order, same order inside a group; 0 = up-right diagonal, 1 = horizontal, 2 = vertical.
-__device__ __forceinline__ int scan_pos_small(int scan_idx, int dim_log2, int idx)   // dim 1,2,4,8 (log2 0..3)
-{
-  const int dim = 1 << dim_log2;
-  if (scan_idx == 1) return idx;                                              // (y = idx / dim, x = idx % dim)
-  if (scan_idx == 2) return (idx & (dim - 1)) * dim + (idx >> dim_log2);      // x = idx / dim, y = idx % dim
-  // diagonal: walk anti-diagonals d = x + y from bottom-left (max y) to top-right
-  int d = 0, start = 0;
-  for (;; ++d) {
-    const int ylo = max(0, d - (dim - 1)), yhi = min(d, dim - 1), len = yhi - ylo + 1;
-    if (idx < start + len) { const int y = yhi - (idx - start); return y * dim + (d - y); }
-    start += len;
-  }
-}
+// visited in scan order (scan_small), same order inside a group
 __device__ __forceinline__ int scan_pos(int scan_idx, int log2_n, int idx)
 {
-  if (log2_n <= 2) return scan_pos_small(scan_idx, log2_n, idx);
+  if (log2_n <= 2) return scan_small(scan_idx, log2_n, idx);
   const int n = 1 << log2_n;
-  const int cg = scan_pos_small(scan_idx, log2_n - 2, idx >> 4);              // group (y*(n/4) + x)
-  const int in = scan_pos_small(scan_idx, 2, idx & 15);
+  const int cg = scan_small(scan_idx, log2_n - 2, idx >> 4);                  // group (y*(n/4) + x)
+  const int in = scan_small(scan_idx, 2, idx & 15);
   const int gw = n >> 2;
   return ((cg / gw) * 4 + (in >> 2)) * n + (cg % gw) * 4 + (in & 3);
 }
