@@ -62,8 +62,17 @@ COEFF_HD uint8_t cabac_next_lps(int uc)
   return (uint8_t)((trans[s] << 1) | (s == 0 ? 1 - mps : mps));
 }
 
-COEFF_FN int quant_scale(int r) { const int t[6] = { COEFF_QUANT_SCALES }; return t[r]; }
-COEFF_FN int inv_quant_scale(int r) { const int t[6] = { COEFF_INV_QUANT_SCALES }; return t[r]; }
+// Six 16-bit table entries packed into two 64-bit immediates, looked up with shifts: a small array indexed at run time
+// is built in local memory (the thread's stack) on every use.
+struct Pack6x16 { unsigned long long lo, hi; };
+COEFF_HD constexpr Pack6x16 pack6x16(int a, int b, int c, int d, int e, int f)
+{
+  return { (unsigned long long)a | (unsigned long long)b << 16 | (unsigned long long)c << 32 | (unsigned long long)d << 48,
+           (unsigned long long)e | (unsigned long long)f << 16 };
+}
+COEFF_HD int unpack6x16(Pack6x16 p, int r) { return (int)(((r < 4 ? p.lo : p.hi) >> (16 * (r & 3))) & 0xffff); }
+COEFF_FN int quant_scale(int r) { constexpr Pack6x16 t = pack6x16(COEFF_QUANT_SCALES); return unpack6x16(t, r); }
+COEFF_FN int inv_quant_scale(int r) { constexpr Pack6x16 t = pack6x16(COEFF_INV_QUANT_SCALES); return unpack6x16(t, r); }
 
 // kvz_get_scaled_qp (transform.c:56-62, 88-102) with the chroma QP mapping table folded into its rule; qp_offset is
 // the bit depth's 6 * (bitdepth - 8).  type: 0 luma, else chroma.
@@ -75,7 +84,7 @@ COEFF_HD int scaled_qp(int type, int qp, int qp_offset)
   int c;
   if (q < 30) c = q;
   else if (q >= 44) c = q - 6;
-  else { const int mid[14] = { 29, 30, 31, 32, 33, 33, 34, 34, 35, 35, 36, 36, 37, 37 }; c = mid[q - 30]; }
+  else c = q < 34 ? q - 1 : 33 + ((q - 34) >> 1);      // 29, 30, 31, 32, 33, 33, 34, 34, 35, 35, 36, 36, 37, 37
   return c + qp_offset;
 }
 

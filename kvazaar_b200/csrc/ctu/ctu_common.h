@@ -52,6 +52,20 @@ extern __shared__ __align__(16) unsigned char ctu_smem_raw[];
 #endif
 #define CTU_LEADER if (CTU_TID == CTU_LEADER_TID)
 
+// Shared-window addressing.  Inside a __noinline__ function ptxas cannot see where a pointer argument points, so loads
+// and stores through it are generic (LD / ST: the L1TEX path and its long scoreboard) even when every caller passes
+// shared memory.  sm(p) re-derives such a pointer from the shared-memory symbol: accesses through the result compile to
+// LDS / STS, and it costs one or two integer operations.  Only for objects that are ALWAYS in the CTA's shared memory
+// (CtuST and what is carved out of it); the identity in the host build.
+#if defined(__CUDA_ARCH__)
+template <typename T> CTU_FN T *sm(T *p)
+{
+  return reinterpret_cast<T *>(ctu_smem_raw + (reinterpret_cast<const unsigned char *>(p) - ctu_smem_raw));
+}
+#else
+template <typename T> CTU_FN T *sm(T *p) { return p; }
+#endif
+
 // Frame-level data (reconstruction planes, CU records, border buffers, SAO parameters, row context models) is written
 // by the CTA of one CTU and read by the CTAs of its neighbours, which run on other SMs inside the same launch: such
 // loads must be served by L2 (ld.global.cg), never by a possibly stale line of this SM's L1.

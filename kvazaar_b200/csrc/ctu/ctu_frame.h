@@ -655,7 +655,10 @@ template <typename Pix> CTU_FN_NOINLINE void enc_coding_tree(const EncTrack<Pix>
 template <typename Pix> CTU_FN_NOINLINE void ctu_track_models(const CtxT<Pix> &c, const FrameDevT<Pix> *F, int cx, int cy)
 {
   CTU_LEADER {
-    CabacState cs = c.S->cabac0;
+    // the models are walked in the search's spare copy (shared memory; the search is over): cost walks that adapt
+    // them read and write shared memory, not the leader's stack
+    CabacState &cs = c.S->tmp;
+    cs = c.S->cabac0;
     cs.update = 1;
     if (c.cfg->sao_type) {
       const SaoRec *sl = &F->sao[2 * (cy * F->wlcu + cx)], *sc = sl + 1;

@@ -59,7 +59,7 @@ struct Team { int tid, nt, warp; unsigned mask; };
 CTU_FN Team team_cta() { Team t = { (int)threadIdx.x, (int)blockDim.x, 0, 0xffffffffu }; return t; }
 CTU_FN Team team_warp() { Team t = { (int)(threadIdx.x & 31), 32, 1, 0xffffffffu }; return t; }
 CTU_FN Team team_half() { Team t = { (int)(threadIdx.x & 15), 16, 1, 0xffffu << (threadIdx.x & 16) }; return t; }
-CTU_FN void tsync(const Team &t) { if (t.warp) __syncwarp(t.mask); else __syncthreads(); }
+CTU_FN void tsync(Team t) { if (t.warp) __syncwarp(t.mask); else __syncthreads(); }
 #define CTU_NWARPS ((int)(blockDim.x >> 5))
 #define CTU_WARP ((int)(threadIdx.x >> 5))
 #define CTU_HALF ((int)(threadIdx.x >> 4))
@@ -67,7 +67,7 @@ CTU_FN void tsync(const Team &t) { if (t.warp) __syncwarp(t.mask); else __syncth
 CTU_FN Team team_cta() { Team t = { 0, 1, 0, 0 }; return t; }
 CTU_FN Team team_warp() { Team t = { 0, 1, 1, 0 }; return t; }
 CTU_FN Team team_half() { Team t = { 0, 1, 1, 0 }; return t; }
-CTU_FN void tsync(const Team &) {}
+CTU_FN void tsync(Team) {}
 #define CTU_NWARPS 1
 #define CTU_WARP 0
 #define CTU_HALF 0
@@ -191,7 +191,10 @@ template <typename Pix> CTU_FN Plane<Pix> plane_of(CtuWorkT<Pix> *W, LcuLevel<Pi
 // The [1 2 1] smoothing of the luma references and the DC sum of every colour in `mask`, from the unfiltered references
 // r[colour].top / .left of blocks of log2w[colour] (the tail of build_refs_multi).  n0: the number of luma references
 // per edge, 2 * (1 << log2w[0]) + 1, or 0 when `mask` has no luma.
-template <typename Pix> CTU_FN void refs_smooth_dc(const int log2w[3], int mask, int n0, IntraRefs<Pix> *r)
+// l2p: log2w[colour] packed four bits per colour (a small array indexed by colour would live in local memory)
+CTU_FN int pack_log2w(int l0, int l1, int l2) { return l0 | (l1 << 4) | (l2 << 8); }
+CTU_FN int log2w_of(int l2p, int color) { return (l2p >> (4 * color)) & 15; }
+template <typename Pix> CTU_FN void refs_smooth_dc_p(int l2p, int mask, int n0, IntraRefs<Pix> *r)
 {
   // smoothing of the luma references; one thread per colour sums the DC
   #pragma unroll 1
@@ -199,10 +202,10 @@ template <typename Pix> CTU_FN void refs_smooth_dc(const int log2w[3], int mask,
     if (i >= 2 * n0) {
       const int color = i - 2 * n0;
       if ((mask >> color) & 1) {
-        const int w = 1 << log2w[color];
+        const int w = 1 << log2w_of(l2p, color);
         int s = 0;
         for (int k = 1; k <= w; ++k) s += r[color].top[k] + r[color].left[k];
-        r[color].dc = (s + w) >> (log2w[color] + 1);
+        r[color].dc = (s + w) >> (log2w_of(l2p, color) + 1);
       }
       continue;
     }
@@ -217,19 +220,25 @@ template <typename Pix> CTU_FN void refs_smooth_dc(const int log2w[3], int mask,
   }
   CTU_SYNC();
 }
+template <typename Pix> CTU_FN void refs_smooth_dc(const int log2w[3], int mask, int n0, IntraRefs<Pix> *r)
+{
+  refs_smooth_dc_p(pack_log2w(log2w[0], log2w[1], log2w[2]), mask, n0, r);
+}
 
 // kvz_intra_build_reference for the blocks of the colours in `mask` (bit per colour) at luma position (x, y) (picture
 // coordinates), into r[colour], followed by the [1 2 1] smoothing (done eagerly: the reference's lazy flag only saves
-// time; chroma never reads it) and the DC sum.  log2w[colour]: the block sizes.  One pass over all colours: the border
+// time; chroma never reads it) and the DC sum.  l2p: the block sizes (pack_log2w); r: S->refs.  One pass over all colours: the border
 // reads of the three planes overlap instead of queueing behind each other.
-template <typename Pix> CTU_FN_NOINLINE void build_refs_multi(const SmTables *T, const CtuConfig *cfg, CtuWorkT<Pix> *W, LcuLevel<Pix> *L, const int log2w[3], int mask, int x, int y, IntraRefs<Pix> *r)
+template <typename Pix> CTU_FN_NOINLINE void build_refs_multi(const SmTables *T0, int width, int height, CtuWorkT<Pix> *W, LcuLevel<Pix> *L, int l2p, int mask, int x, int y, IntraRefs<Pix> *r0)
 {
+  const SmTables *T = sm(T0);
+  IntraRefs<Pix> *r = sm(r0);
   const int lx = x & 63, ly = y & 63;
   const bool has_left = x > 0, has_top = y > 0, inner = has_left && has_top;
   const int mid = 1 << (PixDepth<Pix>::bd - 1);       // value of unavailable references (ref: intra.c:319)
   int n_of[3], start[4];
   start[0] = 0;
-  for (int col = 0; col < 3; ++col) { n_of[col] = ((mask >> col) & 1) ? 2 * (1 << log2w[col]) + 1 : 0; start[col + 1] = start[col] + 2 * n_of[col]; }
+  for (int col = 0; col < 3; ++col) { n_of[col] = ((mask >> col) & 1) ? 2 * (1 << log2w_of(l2p, col)) + 1 : 0; start[col + 1] = start[col] + 2 * n_of[col]; }
   #pragma unroll 1
   for (int it = CTU_TID; it < start[3]; it += CTU_NT) {
     const int color = it >= start[2] ? 2 : (it >= start[1] ? 1 : 0);
@@ -238,8 +247,8 @@ template <typename Pix> CTU_FN_NOINLINE void build_refs_multi(const SmTables *T,
     const Plane<Pix> P = plane_of(W, L, color);
     const int px = lx >> is_c, py = ly >> is_c, lw = P.lw;
     int al = 0, at = 0;
-    if (has_left) { al = T->ref_left[ly >> 2][lx >> 2] >> is_c; al = imin(al, 2 * w); al = imin(al, (cfg->height - y) >> is_c); }
-    if (has_top) { at = T->ref_top[ly >> 2][lx >> 2] >> is_c; at = imin(at, 2 * w); at = imin(at, (cfg->width - x) >> is_c); }
+    if (has_left) { al = T->ref_left[ly >> 2][lx >> 2] >> is_c; al = imin(al, 2 * w); al = imin(al, (height - y) >> is_c); }
+    if (has_top) { at = T->ref_top[ly >> 2][lx >> 2] >> is_c; at = imin(at, 2 * w); at = imin(at, (width - x) >> is_c); }
     // the _inner variant copies in groups of four, at least one group (intra.c:486-494, 512-516)
     const int nl = inner ? imax(4, (al + 3) & ~3) : al;
     const int ntp = inner ? imax(4, (at + 3) & ~3) : at;
@@ -264,15 +273,27 @@ template <typename Pix> CTU_FN_NOINLINE void build_refs_multi(const SmTables *T,
     (is_top ? r[color].top : r[color].left)[e] = (Pix)v;
   }
   CTU_SYNC();
-  refs_smooth_dc(log2w, mask, n_of[0], r);
+  refs_smooth_dc_p(l2p, mask, n_of[0], r);
 }
 template <typename Pix> CTU_FN void build_refs(const SmTables *T, const CtuConfig *cfg, CtuWorkT<Pix> *W, LcuLevel<Pix> *L, int log2w, int color, int x, int y, IntraRefs<Pix> *r)
 {
-  int l[3] = { log2w, log2w, log2w };
-  build_refs_multi(T, cfg, W, L, l, 1 << color, x, y, r - color);
+  build_refs_multi(T, cfg->width, cfg->height, W, L, pack_log2w(log2w, log2w, log2w), 1 << color, x, y, r - color);
 }
 
 // ------------------------------------------------------------------------------------------------ intra prediction
+// The sample displacement and its inverse for an angular mode at |mode - 26| (vertical) / |10 - mode| (horizontal) =
+// adisp, 0..8 (modedisp2sampledisp, modedisp2invsampledisp: intra-generic.c:59-60), as immediates packed into 64-bit
+// words: a 9-entry array indexed at run time would be built in local memory on every use, inside the per-sample loops.
+CTU_FN int ang_disp(int adisp)          // 0, 2, 5, 9, 13, 17, 21, 26, 32
+{
+  return adisp == 8 ? 32 : (int)((0x1A15110D09050200ull >> (8 * adisp)) & 0xff);
+}
+CTU_FN int ang_inv(int adisp)           // 0, 4096, 1638, 910, 630, 482, 390, 315, 256
+{
+  if (adisp == 8) return 256;
+  const uint64_t w = adisp < 4 ? 0x038E066610000000ull : 0x013B018601E20276ull;
+  return (int)((w >> (16 * (adisp & 3))) & 0xffff);
+}
 template <typename Pix> CTU_FN int ang_ref(const Pix *rmain, const Pix *rside, int idx, int inv)
 {
   if (idx >= -1) return rmain[idx + 1];
@@ -281,19 +302,17 @@ template <typename Pix> CTU_FN int ang_ref(const Pix *rmain, const Pix *rside, i
 }
 template <typename Pix> CTU_FN int angular_px(int mode, const Pix *top, const Pix *left, int ox, int oy)
 {
-  const int disp_tab[9] = { 0, 2, 5, 9, 13, 17, 21, 26, 32 };
-  const int inv_tab[9] = { 0, 4096, 1638, 910, 630, 482, 390, 315, 256 };
   const bool vertical = mode >= 18;
   const int mdisp = vertical ? mode - 26 : 10 - mode;
   const int adisp = iabs(mdisp);
-  const int sdisp = mdisp < 0 ? -disp_tab[adisp] : disp_tab[adisp];
+  const int sdisp = mdisp < 0 ? -ang_disp(adisp) : ang_disp(adisp);
   const Pix *rmain = vertical ? top : left;
   const Pix *rside = vertical ? left : top;
   const int x = vertical ? ox : oy, y = vertical ? oy : ox;
   if (sdisp == 0) return rmain[x + 1];
   const int pos = (y + 1) * sdisp;
   const int di = pos >> 5, df = pos & 31;
-  const int inv = inv_tab[adisp];
+  const int inv = ang_inv(adisp);
   const int r1 = ang_ref(rmain, rside, x + di, inv);
   if (df == 0) return r1;
   const int r2 = ang_ref(rmain, rside, x + di + 1, inv);
@@ -394,13 +413,11 @@ static_assert(sizeof(RoughExt<uint16_t>) <= CTU_ARENA_BYTES, "rough-search scrat
 
 CTU_FN void ang_params(int mode, bool *vertical, int *sdisp, int *inv)
 {
-  const int disp_tab[9] = { 0, 2, 5, 9, 13, 17, 21, 26, 32 };
-  const int inv_tab[9] = { 0, 4096, 1638, 910, 630, 482, 390, 315, 256 };
   *vertical = mode >= 18;
   const int mdisp = *vertical ? mode - 26 : 10 - mode;
   const int adisp = iabs(mdisp);
-  *sdisp = mdisp < 0 ? -disp_tab[adisp] : disp_tab[adisp];
-  *inv = inv_tab[adisp];
+  *sdisp = mdisp < 0 ? -ang_disp(adisp) : ang_disp(adisp);
+  *inv = ang_inv(adisp);
 }
 
 // difference block (prediction - source) of the w8 x w8 sub-block at (bx, by) of mode m into d[], row-major, in the
@@ -544,9 +561,14 @@ CTU_FN int dot4_s16_s8(const int16_t *s, const int8_t *m, int acc) { return acc 
 
 // forward: dst[k*N + j] = (int16)((sum_i M[k][i] * src[j*N + i] + add) >> shift)
 // L2N != 0: the size is a compile-time constant (the 4x4 path: most transform units of a CTU)
+// The transform-unit path below works on shared memory only: the team's arena slot, SmTables, the models in CtuST.  Its
+// functions take the team, the scratch and the job by value and re-derive their pointers with sm().
 template <int L2N>
-CTU_FN_NOINLINE void fwd_pass(const Team &tm, const int16_t *src, int16_t *dst, const int8_t *M, int n_rt, int shift)
+CTU_FN_NOINLINE void fwd_pass(Team tm, const int16_t *src0, int16_t *dst0, const int8_t *M0, int n_rt, int shift)
 {
+  const int16_t *src = sm(src0);
+  int16_t *dst = sm(dst0);
+  const int8_t *M = sm(M0);
   const int add = 1 << (shift - 1);
   const int n = L2N ? (1 << L2N) : n_rt;
   const int log2n = L2N ? L2N : (n == 4 ? 2 : (n == 8 ? 3 : (n == 16 ? 4 : 5)));
@@ -563,8 +585,11 @@ CTU_FN_NOINLINE void fwd_pass(const Team &tm, const int16_t *src, int16_t *dst, 
 }
 // inverse: dst[j*N + k] = clip16((sum_i M[i][k] * src[i*N + j] + add) >> shift)
 template <int L2N>
-CTU_FN_NOINLINE void inv_pass(const Team &tm, const int16_t *src, int16_t *dst, const int8_t *M, int n_rt, int shift)
+CTU_FN_NOINLINE void inv_pass(Team tm, const int16_t *src0, int16_t *dst0, const int8_t *M0, int n_rt, int shift)
 {
+  const int16_t *src = sm(src0);
+  int16_t *dst = sm(dst0);
+  const int8_t *M = sm(M0);
   const int add = 1 << (shift - 1);
   const int n = L2N ? (1 << L2N) : n_rt;
   const int log2n = L2N ? L2N : (n == 4 ? 2 : (n == 8 ? 3 : (n == 16 ? 4 : 5)));
@@ -618,10 +643,12 @@ CTU_FN void quant_sign_hide_group(const SmTables *T, const int16_t *coef, int16_
 }
 
 // kvz_quant: b -> q (intra slice: rounding offset 171)
-template <typename Pix> CTU_FN_NOINLINE void quant_block(const Team &tm, const SmTables *T, const CtuConfig *cfg, const TuS<Pix> &tu, int n, int type, int scan_idx)
+template <typename Pix> CTU_FN_NOINLINE void quant_block(Team tm, const SmTables *T0, int qp, bool signhide, TuS<Pix> tu, int n, int type, int scan_idx)
 {
+  const SmTables *T = sm(T0);
+  tu.base = sm(tu.base);
   const int log2n = ilog2(n);
-  const int qp_scaled = scaled_qp_px<Pix>(type, cfg->qp);
+  const int qp_scaled = scaled_qp_px<Pix>(type, qp);
   const int qc = quant_scale(qp_scaled % 6);
   const int transform_shift = 15 - PixDepth<Pix>::bd - log2n;
   const int q_bits = 14 + qp_scaled / 6 + transform_shift;
@@ -645,7 +672,7 @@ template <typename Pix> CTU_FN_NOINLINE void quant_block(const Team &tm, const S
   }
   if (ac) CTU_ATOMIC_ADD(&fx->ac_sum, ac);
   tsync(tm);
-  if (!cfg->signhide_enable || fx->ac_sum < 2) return;
+  if (!signhide || fx->ac_sum < 2) return;
   const int num_cg = (n * n) >> 4;
   int32_t *cg_nz = tu.cg_nzflag();
   #pragma unroll 1
@@ -663,11 +690,12 @@ template <typename Pix> CTU_FN_NOINLINE void quant_block(const Team &tm, const S
 
 // kvz_dequant: q -> b.  type: 0 luma, 2 / 3 chroma
 template <int L2N, typename Pix>
-CTU_FN_NOINLINE void dequant_block(const Team &tm, const CtuConfig *cfg, const TuS<Pix> &tu, int n_rt, int type)
+CTU_FN_NOINLINE void dequant_block(Team tm, int qp, TuS<Pix> tu, int n_rt, int type)
 {
+  tu.base = sm(tu.base);
   const int n = L2N ? (1 << L2N) : n_rt;
   const int transform_shift = 15 - PixDepth<Pix>::bd - (L2N ? L2N : ilog2(n));
-  const int qp_scaled = scaled_qp_px<Pix>(type, cfg->qp);
+  const int qp_scaled = scaled_qp_px<Pix>(type, qp);
   const int shift = 20 - 14 - transform_shift;
   const int scale = inv_quant_scale(qp_scaled % 6) << (qp_scaled / 6);
   const int add = 1 << (shift - 1);
@@ -681,13 +709,14 @@ CTU_FN_NOINLINE void dequant_block(const Team &tm, const CtuConfig *cfg, const T
 
 // ------------------------------------------------------------------------------------------------ RDOQ
 // kvz_rdoq_sign_hiding on the unit's rate tables (a call of its own: RDOQ's lanes wait while the leader runs it)
-template <typename Pix> CTU_FN_NOINLINE void rdoq_sign_hiding(const TuS<Pix> &tu, const uint16_t *blk, double lambda, int qp_scaled, int last_pos, const int16_t *coef, int16_t *q)
+template <typename Pix> CTU_FN_NOINLINE void rdoq_sign_hiding(TuS<Pix> tu, const uint16_t *blk, double lambda, int qp_scaled, int last_pos, const int16_t *coef, int16_t *q)
 {
-  kvzcoeff::rdoq_sign_hiding(tu.inc(), tu.dec(), tu.sig_inc(), tu.qdelta(), blk, lambda, PixDepth<Pix>::bd, qp_scaled, last_pos, coef, q);
+  tu.base = sm(tu.base);
+  kvzcoeff::rdoq_sign_hiding(tu.inc(), tu.dec(), tu.sig_inc(), tu.qdelta(), sm(blk), lambda, PixDepth<Pix>::bd, qp_scaled, last_pos, sm(coef), sm(q));
 }
 
 // RDOQ runs on the first nl = rdoq_lanes() threads of a team (the first warp of a CTA team), whose lanes are `mask`
-CTU_FN int rdoq_lanes(const Team &t) { return t.nt < CTU_TEAM_N ? t.nt : CTU_TEAM_N; }
+CTU_FN int rdoq_lanes(Team t) { return t.nt < CTU_TEAM_N ? t.nt : CTU_TEAM_N; }
 #if defined(__CUDA_ARCH__)
 CTU_FN void rq_sync(unsigned mask) { __syncwarp(mask); }
 CTU_FN int team_max(int v, unsigned mask, int nl) { for (int o = nl >> 1; o > 0; o >>= 1) v = max(v, __shfl_xor_sync(mask, v, o)); return v; }
@@ -701,9 +730,12 @@ CTU_FN int team_sum(int v, unsigned, int) { return v; }
 // kvz_rdoq for one TU, executed by the RDOQ lanes of a team (lane < nl): coef = tu->b, levels to tu->q.  `cabac` = the
 // models of state->cabac (NOT the search copy: rdo.c:665).  type 0 luma / 2 chroma; tr_depth as in quant-generic.c:237-238.
 template <int L2N, typename Pix>
-CTU_FN_NOINLINE void rdoq_team(const SmTables *T, const SmTables *tb, const CtuConfig *cfg, const uint8_t *cabac, const TuS<Pix> &tu, int log2n_rt, int type,
+CTU_FN_NOINLINE void rdoq_team(const SmTables *T0, const uint8_t *cabac0, int qp, double lambda, bool SH, TuS<Pix> tu, int log2n_rt, int type,
                       int scan_idx, int tr_depth, int lane, int nl, unsigned mask)
 {
+  const SmTables *T = sm(T0);
+  const uint8_t *cabac = sm(cabac0);
+  tu.base = sm(tu.base);
   const int log2n = L2N ? L2N : log2n_rt;
   const int16_t *coef = tu.b();
   int16_t *q = tu.q();
@@ -714,18 +746,16 @@ CTU_FN_NOINLINE void rdoq_team(const SmTables *T, const SmTables *tb, const CtuC
   uint16_t *s_cg_nz = tu.cg_nz();
   const int n = 1 << log2n, nn = n * n;
   const int transform_shift = 15 - PixDepth<Pix>::bd - log2n;
-  const int qp_scaled = scaled_qp_px<Pix>(type, cfg->qp);
+  const int qp_scaled = scaled_qp_px<Pix>(type, qp);
   const int q_bits = 14 + qp_scaled / 6 + transform_shift;
   const int qc = quant_scale(qp_scaled % 6);
   const int half = 1 << (q_bits - 1);
-  const double lambda = cfg->lambda;
-  const bool SH = cfg->signhide_enable != 0;
   // error scale (scalinglist.c:351-368): 2^15 * 2^(-2 * transform_shift) / q / q / 2^(2 * (bd - 8))
   double err_scale = 32768.0;
   for (int i = 0; i < 2 * transform_shift; ++i) err_scale *= 0.5;
   for (int i = 0; i > 2 * transform_shift; --i) err_scale *= 2.0;
   err_scale = err_scale / qc / qc / (1 << (2 * (PixDepth<Pix>::bd - 8)));
-  const RdoqModels m = rdoq_models(cabac, tb->ebits, type);
+  const RdoqModels m = rdoq_models(cabac, T->ebits, type);
   auto sig_cost_of = [&](uint8_t code) { return (code >> 6) == 2 ? 0.0 : lambda * ebits(m, m.sig[code & 63], code >> 6); };
   auto level0_cost = [&](int blk) { const double e = (double)imin(iabs((int)coef[blk]) * qc, 0x7FFFFFFF - half); return e * e * err_scale; };
   const uint16_t *blk_of = sm_scan(T, scan_idx, log2n - 2);
@@ -990,18 +1020,19 @@ CTU_FN void cabac_bin(const SmTables *tb, CabacState *c, int off, int val, doubl
 
 // kvz_get_coeff_cost's CABAC branch = kvz_encode_coeff_nxn in counting mode on a copy of the search models that is
 // kept when `update` is set (ref: rdo.c:223-264).  Leader only.  The cost estimate codes tr_skip as 0 (rdo.c:251-258);
-// the tracker of the real coder's models passes the TU's flag.  Tables from shared memory (coeff_bits' policy).
+// the tracker of the real coder's models passes the TU's flag.  Tables and models from shared memory (coeff_bits'
+// policy; the coefficients may be in either space).
 struct CtuCostWalk {
   const SmTables *T, *tb;
-  const CtuConfig *cfg;
   CabacState *c;
+  bool ts_enable, sh_enable;
   CTU_MFN const uint16_t *scan(int scan_idx, int log2n) const { return sm_scan(T, scan_idx, log2n - 2); }
   CTU_MFN const uint8_t *scan_cg(int scan_idx, int log2n) const { return T->scan_cg[scan_idx][log2n - 2]; }
   CTU_MFN int group_idx(int x) const { return T->group_idx[x]; }
   CTU_MFN const uint8_t *sig_ctx4() const { return T->sig_ctx4; }
   CTU_MFN int32_t *abs_scratch() const { return tb->abs_scratch[CTU_HALF & 7]; }
-  CTU_MFN bool trskip_enable() const { return cfg->trskip_enable; }
-  CTU_MFN bool signhide() const { return cfg->signhide_enable; }
+  CTU_MFN bool trskip_enable() const { return ts_enable; }
+  CTU_MFN bool signhide() const { return sh_enable; }
   CTU_MFN void bin(int off, int val, long long *bits) const
   {
     const uint8_t st = c->ctx[off];
@@ -1012,7 +1043,7 @@ struct CtuCostWalk {
 CTU_FN_NOINLINE double coeff_cost_serial(const SmTables *T, const SmTables *tb, const CtuConfig *cfg, CabacState *c, const int16_t *coeff, int log2n, int type, int scan_idx, int tr_skip,
                                          uint64_t known_cg_mask = COEFF_NO_MASK)
 {
-  CtuCostWalk w = { T, tb, cfg, c };
+  CtuCostWalk w = { sm(T), sm(tb), sm(c), cfg->trskip_enable != 0, cfg->signhide_enable != 0 };
   return (double)coeff_bits(w, coeff, log2n, type, scan_idx, tr_skip, known_cg_mask) * (1.0 / 32768.0);
 }
 
@@ -1031,9 +1062,11 @@ template <typename Pix> struct TuJob {
 };
 
 template <int L2N, typename Pix>
-CTU_FN_NOINLINE void tu_core_t(const Team &tm, const SmTables *T, const SmTables *tb, const CtuConfig *cfg, const uint8_t *cabac0, const TuS<Pix> &tu,
-                               const TuJob<Pix> &j, bool use_trskip)
+CTU_FN_NOINLINE void tu_core_t(Team tm, const SmTables *T0, const CtuConfig *cfg, const uint8_t *cabac0, TuS<Pix> tu, TuJob<Pix> j, bool use_trskip)
 {
+  const SmTables *T = sm(T0);
+  tu.base = sm(tu.base);
+  j.refs = sm(j.refs);
   const int log2n = L2N ? L2N : j.log2n, n = 1 << log2n, nn = n * n;
   const int color = j.color;
   const int ts_shift = 15 - PixDepth<Pix>::bd - log2n;
@@ -1062,10 +1095,10 @@ CTU_FN_NOINLINE void tu_core_t(const Team &tm, const SmTables *T, const SmTables
   const int type = color == 0 ? 0 : 2;
   if (cfg->rdoq_enable && (n > 4 || !cfg->rdoq_skip)) {
     const int nl = rdoq_lanes(tm);
-    if (tm.tid < nl) rdoq_team<L2N>(T, tb, cfg, cabac0, tu, log2n, type, j.scan_idx, j.rdoq_tr_depth, tm.tid, nl, tm.mask);
+    if (tm.tid < nl) rdoq_team<L2N>(T, cabac0, cfg->qp, cfg->lambda, cfg->signhide_enable != 0, tu, log2n, type, j.scan_idx, j.rdoq_tr_depth, tm.tid, nl, tm.mask);
     tsync(tm);
   } else {
-    quant_block(tm, T, cfg, tu, n, type, j.scan_idx);
+    quant_block(tm, T, cfg->qp, cfg->signhide_enable != 0, tu, n, type, j.scan_idx);
   }
   {
     uint32_t m0 = 0, m1 = 0;
@@ -1084,7 +1117,7 @@ CTU_FN_NOINLINE void tu_core_t(const Team &tm, const SmTables *T, const SmTables
   tsync(tm);
   int ssd = 0;
   if (fx->has) {
-    dequant_block<L2N>(tm, cfg, tu, n, color == 0 ? 0 : (color == 1 ? 2 : 3));
+    dequant_block<L2N>(tm, cfg->qp, tu, n, color == 0 ? 0 : (color == 1 ? 2 : 3));
     if (use_trskip) {
       const int offs = 1 << (ts_shift - 1);
       #pragma unroll 1
@@ -1122,19 +1155,21 @@ CTU_FN_NOINLINE void tu_core_t(const Team &tm, const SmTables *T, const SmTables
   }
 }
 
-template <typename Pix> CTU_FN void tu_core(const Team &tm, const SmTables *T, const SmTables *tb, const CtuConfig *cfg, const uint8_t *cabac0, const TuS<Pix> &tu,
+template <typename Pix> CTU_FN void tu_core(Team tm, const SmTables *T, const SmTables *tb, const CtuConfig *cfg, const uint8_t *cabac0, TuS<Pix> tu,
                     const TuJob<Pix> &j, bool use_trskip)
 {
-  if (j.log2n == 2) tu_core_t<2>(tm, T, tb, cfg, cabac0, tu, j, use_trskip);
-  else tu_core_t<0>(tm, T, tb, cfg, cabac0, tu, j, use_trskip);
+  (void)tb;      // the same SmTables as T in every caller
+  if (j.log2n == 2) tu_core_t<2>(tm, T, cfg, cabac0, tu, j, use_trskip);
+  else tu_core_t<0>(tm, T, cfg, cabac0, tu, j, use_trskip);
 }
 
 // One colour of one transform unit including the transform-skip decision of 4x4 luma units
 // (kvz_quantize_residual_trskip, ref: transform.c:242-288).  `sc`: the search models the decision's bit costs read.
 // Returns tr_skip (uniform over the team); the chosen alternative is in tu.q() / tu.rec() / fx->has / fx->ssd.
-template <typename Pix> CTU_FN_NOINLINE int tu_eval(const Team &tm, const SmTables *T, const SmTables *tb, const CtuConfig *cfg, const uint8_t *cabac0, CabacState *sc,
-                            const TuS<Pix> &tu, const TuJob<Pix> &j)
+template <typename Pix> CTU_FN_NOINLINE int tu_eval(Team tm, const SmTables *T, const SmTables *tb, const CtuConfig *cfg, const uint8_t *cabac0, CabacState *sc,
+                            TuS<Pix> tu, TuJob<Pix> j)
 {
+  tu.base = sm(tu.base);
   if (!(j.log2n == 2 && j.color == 0 && cfg->trskip_enable)) {
     tu_core(tm, T, tb, cfg, cabac0, tu, j, false);
     return 0;

@@ -45,7 +45,7 @@ template <typename Pix> struct CtuST {                       // per-CTA scalar s
   int32_t pad0[3];
   CabacState cabac0;                // state->cabac: the real coder's models when the CTU starts (constant)
   CabacState sc;                    // state->search_cabac
-  CabacState tmp;                   // temp_cabac of the combined-CU path (search.c:989)
+  CabacState tmp;                   // temp_cabac of the combined-CU path (search.c:989); after the search: ctu_track_models' models
   SearchFrame fr[5];
   double ret_cost;
   IntraRefs<Pix> refs[3];
@@ -293,8 +293,7 @@ template <typename Pix> CTU_FN_NOINLINE void intra_recon_leaf(const CtxT<Pix> &c
   {
     int need = 0;
     for (int col = first; col <= last; ++col) if (!((refs_valid >> col) & 1)) need |= 1 << col;
-    const int l2[3] = { tu_log2(depth, 0), tu_log2(depth, 1), tu_log2(depth, 2) };
-    if (need) build_refs_multi(&c.S->tb, c.cfg, c.W, L, l2, need, x, y, S->refs);
+    if (need) build_refs_multi(&c.S->tb, c.cfg->width, c.cfg->height, c.W, L, pack_log2w(tu_log2(depth, 0), tu_log2(depth, 1), tu_log2(depth, 2)), need, x, y, S->refs);
   }
   PROF_ADD(S, PR_REFS);
   // cur_pu of quantize_tr_residual: the RDOQ context selector reads its depths before the cbf bits change
@@ -716,8 +715,9 @@ template <typename Pix> CTU_FN_NOINLINE int rough_search_replay(const CtxT<Pix> 
 }
 
 // copy of a transform-unit job's reconstruction and levels (team)
-template <typename Pix> CTU_FN_NOINLINE void keep_unit(const Team &tm, const TuS<Pix> &tu, Pix *kr, int16_t *kq)
+template <typename Pix> CTU_FN_NOINLINE void keep_unit(Team tm, TuS<Pix> tu, Pix *kr, int16_t *kq)
 {
+  tu.base = sm(tu.base);
   const Pix *r = tu.rec();
   const int16_t *q = tu.q();
   #pragma unroll 1
@@ -741,8 +741,7 @@ template <typename Pix> CTU_FN_NOINLINE void search_cu_intra(const CtxT<Pix> &c,
   PROF_T0(PR_REFS);
   {
     // luma for the rough search; the chroma references the CU's reconstruction (and RDO candidates) will need as well
-    const int l2[3] = { log2w, tu_log2(depth, 1), tu_log2(depth, 2) };
-    build_refs_multi(&c.S->tb, cfg, c.W, L, l2, ((x & 4) || (y & 4)) ? 1 : 7, x, y, S->refs);
+    build_refs_multi(&c.S->tb, cfg->width, cfg->height, c.W, L, pack_log2w(log2w, tu_log2(depth, 1), tu_log2(depth, 2)), ((x & 4) || (y & 4)) ? 1 : 7, x, y, S->refs);
   }
   PROF_ADD(S, PR_REFS);
   // rough search: SATD (and SAD for 4x4 transform-skip candidates) of every mode, then the reference's selection

@@ -17,15 +17,22 @@ def run(cmd, **kw):
     return subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True, **kw).stdout
 
 
-def function_of_each_instruction(obj):
+def function_of_each_instruction(obj, with_text=False):
+    """The device function of every SASS instruction of ctu_frame_kernel (both instantiations) in `obj`, an object file
+    or the shared library.  with_text: (kernel instantiation, function, instruction) triples instead, the instantiation
+    being the kernel's template argument as mangled ("h": uint8_t, "t": uint16_t)."""
     with tempfile.TemporaryDirectory() as d:
         subprocess.run(["cuobjdump", "-xelf", "all", os.path.abspath(obj)], cwd=d, stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL)
-        cubin = [f for f in os.listdir(d) if f.endswith(".cubin")][0]
-        dis = run(["nvdisasm", "-c", os.path.join(d, cubin)])
-    names, cur, infn = [], "kernel body", False
+        cubins = sorted(f for f in os.listdir(d) if f.endswith(".cubin"))
+        # a library holds one cubin per translation unit: only the CTU driver's has the kernel
+        cubins = [f for f in cubins if b"ctu_frame_kernel" in open(os.path.join(d, f), "rb").read()]
+        dis = "".join(run(["nvdisasm", "-c", os.path.join(d, f)]) for f in cubins)
+    names, cur, infn, kern = [], "kernel body", False, "?"
     for ln in dis.splitlines():
         if ln.startswith("_ZN") and "ctu_frame_kernel" in ln:
             infn, cur = True, "kernel body"
+            k = re.search(r"ctu_frame_kernelI(\w)E", ln)
+            kern = k.group(1) if k else "?"
             continue
         if ln.startswith("_ZN") and "ctu_frame_kernel" not in ln:
             infn = False
@@ -37,7 +44,7 @@ def function_of_each_instruction(obj):
         if ln.startswith("$_ZN") and "ctu_frame_kernel" not in ln:
             infn = False
         if infn and re.match(r"\s+/\*[0-9a-f]{4,}\*/", ln):
-            names.append(cur)
+            names.append((kern, cur, ln) if with_text else cur)
     return names
 
 
