@@ -56,11 +56,14 @@ extern __shared__ __align__(16) unsigned char ctu_smem_raw[];
 // and stores through it are generic (LD / ST: the L1TEX path and its long scoreboard) even when every caller passes
 // shared memory.  sm(p) re-derives such a pointer from the shared-memory symbol: accesses through the result compile to
 // LDS / STS, and it costs one or two integer operations.  Only for objects that are ALWAYS in the CTA's shared memory
-// (CtuST and what is carved out of it); the identity in the host build.
+// (CtuST and what is carved out of it); the identity in the host build.  The offset is taken with cvta (the shared
+// address of p), not as the difference of two generic pointers: with that form the search spine's build faulted on
+// the device although every pointer it was given lay inside the window.
 #if defined(__CUDA_ARCH__)
 template <typename T> CTU_FN T *sm(T *p)
 {
-  return reinterpret_cast<T *>(ctu_smem_raw + (reinterpret_cast<const unsigned char *>(p) - ctu_smem_raw));
+  const unsigned off = (unsigned)__cvta_generic_to_shared(p) - (unsigned)__cvta_generic_to_shared(ctu_smem_raw);
+  return reinterpret_cast<T *>(ctu_smem_raw + off);
 }
 #else
 template <typename T> CTU_FN T *sm(T *p) { return p; }

@@ -28,11 +28,12 @@ template <typename Pix> struct FrameDevT {
 using FrameDev = FrameDevT<uint8_t>;  // (8-bit alias, see CtuWork)
 
 // ------------------------------------------------------------------------------------------------ init_lcu_t
-template <typename Pix> CTU_FN_NOINLINE void ctu_load(const CtxT<Pix> &c, const FrameDevT<Pix> *F, int cx, int cy)
+template <typename Pix> CTU_FN_NOINLINE void ctu_load(CtuST<Pix> *S, const FrameDevT<Pix> *F, int cx, int cy)
 {
-  const CtuConfig *cfg = c.cfg;
-  CtuWorkT<Pix> *W = c.W;
-  LcuLevel<Pix> *L0 = &c.S->lv[0];
+  S = sm(S);
+  const CtuConfig *cfg = &S->cfg;
+  CtuWorkT<Pix> *W = S->W;
+  LcuLevel<Pix> *L0 = &S->lv[0];
   const int x = cx * 64, y = cy * 64;
   const int Wd = cfg->width, H = cfg->height;
   // FILL(*lcu, 0) for every level of the work tree (work_tree[depth] = work_tree[0] below only differs in the border
@@ -40,7 +41,7 @@ template <typename Pix> CTU_FN_NOINLINE void ctu_load(const CtxT<Pix> &c, const 
   {
     #pragma unroll 1
     for (int d = CTU_TID; d < 5; d += CTU_NT) {
-      LcuLevel<Pix> *L = &c.S->lv[d];
+      LcuLevel<Pix> *L = &S->lv[d];
       LcuStore<Pix> *st = &W->store[d];
       L->rec_y = st->rec_y; L->rec_u = st->rec_u; L->rec_v = st->rec_v;
       L->coeff_y = st->coeff_y; L->coeff_u = st->coeff_u; L->coeff_v = st->coeff_v;
@@ -114,23 +115,24 @@ template <typename Pix> CTU_FN_NOINLINE void ctu_load(const CtxT<Pix> &c, const 
   // work_tree[depth] = work_tree[0]
   for (int d = 1; d <= 4; ++d) {
     const uint32_t *s = (const uint32_t *)L0->cu;
-    uint32_t *p = (uint32_t *)c.S->lv[d].cu;
+    uint32_t *p = (uint32_t *)S->lv[d].cu;
     #pragma unroll 1
     for (int i = CTU_TID; i < (int)(sizeof(L0->cu) / 4); i += CTU_NT) p[i] = s[i];
   }
   // the models the search starts from
   #pragma unroll 1
-  for (int i = CTU_TID; i < (int)(sizeof(CabacState) / 4); i += CTU_NT) ((uint32_t *)&c.S->cabac0)[i] = CTU_LD_FRAME((const uint32_t *)&F->row_ctx[cy] + i);
+  for (int i = CTU_TID; i < (int)(sizeof(CabacState) / 4); i += CTU_NT) ((uint32_t *)&S->cabac0)[i] = CTU_LD_FRAME((const uint32_t *)&F->row_ctx[cy] + i);
   CTU_SYNC();
-  CTU_LEADER { c.S->cabac0.update = 0; c.S->sc = c.S->cabac0; }
+  CTU_LEADER { S->cabac0.update = 0; S->sc = S->cabac0; }
   CTU_SYNC();
 }
 
 // ------------------------------------------------------------------------------------------------ store
-template <typename Pix> CTU_FN_NOINLINE void ctu_store(const CtxT<Pix> &c, const FrameDevT<Pix> *F, int cx, int cy)
+template <typename Pix> CTU_FN_NOINLINE void ctu_store(CtuST<Pix> *S, const FrameDevT<Pix> *F, int cx, int cy)
 {
-  const CtuConfig *cfg = c.cfg;
-  LcuLevel<Pix> *L0 = &c.S->lv[0];
+  S = sm(S);
+  const CtuConfig *cfg = &S->cfg;
+  LcuLevel<Pix> *L0 = &S->lv[0];
   const int x = cx * 64, y = cy * 64, Wd = cfg->width, H = cfg->height;
   const int x_max = imin(x + 64, Wd) - x, y_max = imin(y + 64, H) - y;
   #pragma unroll 1
@@ -238,9 +240,10 @@ template <typename Pix> CTU_FN void dbk_chroma_part(Pix *px, int xs, int ys, int
 }
 
 // kvz_filter_deblock_lcu on the frame planes; all CUs are intra (boundary strength 2), fixed QP
-template <typename Pix> CTU_FN_NOINLINE void ctu_deblock(const CtxT<Pix> &c, const FrameDevT<Pix> *F, int cx, int cy)
+template <typename Pix> CTU_FN_NOINLINE void ctu_deblock(CtuST<Pix> *S, const FrameDevT<Pix> *F, int cx, int cy)
 {
-  const CtuConfig *cfg = c.cfg;
+  S = sm(S);
+  const CtuConfig *cfg = &S->cfg;
   const int Wd = cfg->width, H = cfg->height, Wc = Wd / 2;
   const int x0 = cx * 64, y0 = cy * 64;
   const int end_x = imin(x0 + 64, Wd), end_y = imin(y0 + 64, H);
@@ -411,10 +414,11 @@ template <typename Pix> CTU_FN_NOINLINE int sao_band_offsets(const int32_t bd[2]
 }
 
 // sao_search_best_mode for one component group (luma: planes {0}, chroma: planes {1, 2}).  Leader only.
-template <typename Pix> CTU_FN_NOINLINE void sao_search_best_mode(const CtxT<Pix> &c, const SaoStats *st, int first_plane, int buf_cnt, SaoRec *out, const SaoRec *top, const SaoRec *left, int32_t merge_cost[3])
+template <typename Pix> CTU_FN_NOINLINE void sao_search_best_mode(CtuST<Pix> *S, const SaoStats *st, int first_plane, int buf_cnt, SaoRec *out, const SaoRec *top, const SaoRec *left, int32_t merge_cost[3])
 {
-  const CtuConfig *cfg = c.cfg;
-  const SaoBits sb = { &c.S->tb, c.S->cabac0.ctx };
+  S = sm(S); st = sm(st);
+  const CtuConfig *cfg = &S->cfg;
+  const SaoBits sb = { &S->tb, S->cabac0.ctx };
   const double lambda = cfg->lambda;
   SaoRec edge, band;
   memset(&edge, 0, sizeof(edge)); memset(&band, 0, sizeof(band));
@@ -484,10 +488,11 @@ template <typename Pix> CTU_FN_NOINLINE void sao_search_best_mode(const CtxT<Pix
   }
 }
 
-// kvz_sao_search_lcu; `st` is scratch for the statistics (global or shared)
-template <typename Pix> CTU_FN_NOINLINE void ctu_sao_search(const CtxT<Pix> &c, const FrameDevT<Pix> *F, SaoStats *st, int cx, int cy)
+// kvz_sao_search_lcu; `st` is scratch for the statistics in shared memory (the arena, idle after the search)
+template <typename Pix> CTU_FN_NOINLINE void ctu_sao_search(CtuST<Pix> *S, const FrameDevT<Pix> *F, SaoStats *st, int cx, int cy)
 {
-  const CtuConfig *cfg = c.cfg;
+  S = sm(S); st = sm(st);
+  const CtuConfig *cfg = &S->cfg;
   const int Wd = cfg->width, H = cfg->height;
   const int x0 = cx * 64, y0 = cy * 64;
   const int bw = imin(64, Wd - x0), bh = imin(64, H - y0);
@@ -513,8 +518,8 @@ template <typename Pix> CTU_FN_NOINLINE void ctu_sao_search(const CtxT<Pix> &c, 
     const SaoRec *top_l = cy ? &nb[0] : NULL, *left_l = cx ? &nb[2] : NULL;
     const SaoRec *top_c = top_l ? top_l + 1 : NULL, *left_c = left_l ? left_l + 1 : NULL;
     int32_t mcl[3] = { CTU_MAX_INT, 0, 0 }, mcc[3] = { CTU_MAX_INT, 0, 0 };
-    sao_search_best_mode(c, st, 0, 1, sl, top_l, left_l, mcl);
-    sao_search_best_mode(c, st, 1, 2, sc, top_c, left_c, mcc);
+    sao_search_best_mode(S, st, 0, 1, sl, top_l, left_l, mcl);
+    sao_search_best_mode(S, st, 1, 2, sc, top_c, left_c, mcc);
     sl->merge_up_flag = sl->merge_left_flag = 0;
     if (top_l) {
       if (mcl[2] + mcc[2] <= mcl[0] + mcc[0]) { *sl = *top_l; *sc = *top_c; sl->merge_up_flag = 1; sl->merge_left_flag = 0; }
@@ -537,27 +542,31 @@ CTU_FN void enc_bin(const SmTables *T, uint8_t *ctx, int off, int val)
 
 // All records and coefficients come from level 0 of the work tree: after the search it holds the CTU's decisions (the
 // same values ctu_store wrote to the frame) and the border records of the left / above CTUs (ctu_load).
-template <typename Pix> struct EncTrack { const CtxT<Pix> *c; LcuLevel<Pix> *L0; int x0, y0; CabacState *cs; };
-template <typename Pix> CTU_FN const CuRec *tcu(const EncTrack<Pix> &e, int x, int y) { return cu_at(e.L0, x - e.x0, y - e.y0); }
+// The walk's state is the shared state block (re-derived with sm() in every function): the models in S->tmp, the
+// records and coefficients in S->lv[0].
+template <typename Pix> struct EncTrack { CtuST<Pix> *S; int x0, y0; };
+template <typename Pix> CTU_FN const CuRec *tcu(const EncTrack<Pix> &e, int x, int y) { return cu_at(&e.S->lv[0], x - e.x0, y - e.y0); }
 
 // encode_transform_coeff + encode_transform_unit (ref: encode_coding_tree.c:117-319), context-coded bins only
-template <typename Pix> CTU_FN_NOINLINE void enc_transform_leaf(const EncTrack<Pix> &e, int x, int y, int depth, int tr_depth, int parent_u, int parent_v)
+template <typename Pix> CTU_FN_NOINLINE void enc_transform_leaf(EncTrack<Pix> e, int x, int y, int depth, int tr_depth, int parent_u, int parent_v)
 {
-  const CtxT<Pix> &c = *e.c;
+  CtuST<Pix> *S = e.S = sm(e.S);
+  CabacState *cs = &S->tmp;
+  const LcuLevel<Pix> *L0 = &S->lv[0];
   const CuRec *cur_pu = tcu(e, x, y);
   const CuRec *cur_cu = tcu(e, x & ~7, y & ~7);
   const int cb_y = cbf_is_set(cur_pu->cbf, depth, 0), cb_u = cbf_is_set(cur_cu->cbf, depth, 1), cb_v = cbf_is_set(cur_cu->cbf, depth, 2);
   if (depth < 4) {
-    if (tr_depth == 0 || parent_u) enc_bin(&c.S->tb, e.cs->ctx, CTX_CBF_CHROMA + tr_depth, cb_u);
-    if (tr_depth == 0 || parent_v) enc_bin(&c.S->tb, e.cs->ctx, CTX_CBF_CHROMA + tr_depth, cb_v);
+    if (tr_depth == 0 || parent_u) enc_bin(&S->tb, cs->ctx, CTX_CBF_CHROMA + tr_depth, cb_u);
+    if (tr_depth == 0 || parent_v) enc_bin(&S->tb, cs->ctx, CTX_CBF_CHROMA + tr_depth, cb_v);
   }
-  enc_bin(&c.S->tb, e.cs->ctx, CTX_CBF_LUMA + (tr_depth ? 0 : 1), cb_y);        // CU_INTRA: always signalled
+  enc_bin(&S->tb, cs->ctx, CTX_CBF_LUMA + (tr_depth ? 0 : 1), cb_y);        // CU_INTRA: always signalled
   if (!(cb_y | cb_u | cb_v)) return;
   const int width = 64 >> depth, width_c = depth == 4 ? width : width / 2;
-  e.cs->update = 1;
+  cs->update = 1;
   if (cb_y) {
     const int scan = scan_order_intra(cur_pu->mode, depth);
-    coeff_cost_serial(&c.S->tb, &c.S->tb, c.cfg, e.cs, e.L0->coeff_y + zorder(64, x & 63, y & 63), ilog2(width), 0, scan, cur_pu->tr_skip);
+    coeff_cost_serial(&S->tb, &S->tb, &S->cfg, cs, L0->coeff_y + zorder(64, x & 63, y & 63), ilog2(width), 0, scan, cur_pu->tr_skip);
   }
   int xx = x, yy = y;
   if (depth == 4) {
@@ -569,33 +578,34 @@ template <typename Pix> CTU_FN_NOINLINE void enc_transform_leaf(const EncTrack<P
   if (cu_u || cu_v) {
     const int scan = scan_order_intra(cur_pu->mode_chroma, depth);
     const int zi = zorder(32, (xx >> 1) & 31, (yy >> 1) & 31);
-    if (cu_u) coeff_cost_serial(&c.S->tb, &c.S->tb, c.cfg, e.cs, e.L0->coeff_u + zi, ilog2(width_c), 2, scan, 0);
-    if (cu_v) coeff_cost_serial(&c.S->tb, &c.S->tb, c.cfg, e.cs, e.L0->coeff_v + zi, ilog2(width_c), 2, scan, 0);
+    if (cu_u) coeff_cost_serial(&S->tb, &S->tb, &S->cfg, cs, L0->coeff_u + zi, ilog2(width_c), 2, scan, 0);
+    if (cu_v) coeff_cost_serial(&S->tb, &S->tb, &S->cfg, cs, L0->coeff_v + zi, ilog2(width_c), 2, scan, 0);
   }
 }
 template <typename Pix> CTU_FN void enc_transform_tree(const EncTrack<Pix> &e, int x, int y, int depth)
 {
   // root of the CU's transform tree: tr_depth 0
-  const CtxT<Pix> &c = *e.c;
+  CtuST<Pix> *S = e.S;
   const CuRec *cur_cu = tcu(e, x & ~7, y & ~7);
   const int split = cur_cu->tr_depth > depth;
   if (!split) { enc_transform_leaf(e, x, y, depth, 0, 0, 0); return; }
   // one implicit split (64x64 CU into 32x32 TUs, or NxN into four 4x4 TUs)
   const int cb_u = cbf_is_set(cur_cu->cbf, depth, 1), cb_v = cbf_is_set(cur_cu->cbf, depth, 2);
-  if (depth < 4) { enc_bin(&c.S->tb, e.cs->ctx, CTX_CBF_CHROMA, cb_u); enc_bin(&c.S->tb, e.cs->ctx, CTX_CBF_CHROMA, cb_v); }
+  if (depth < 4) { enc_bin(&S->tb, S->tmp.ctx, CTX_CBF_CHROMA, cb_u); enc_bin(&S->tb, S->tmp.ctx, CTX_CBF_CHROMA, cb_v); }
   const int off = 64 >> (depth + 1);
   for (int k = 0; k < 4; ++k) enc_transform_leaf(e, x + (k & 1) * off, y + (k >> 1) * off, depth + 1, 1, cb_u, cb_v);
 }
 
 // one coding unit (no further split): part mode, intra modes, transform tree
-template <typename Pix> CTU_FN_NOINLINE void enc_coding_unit(const EncTrack<Pix> &e, int x, int y, int depth)
+template <typename Pix> CTU_FN_NOINLINE void enc_coding_unit(EncTrack<Pix> e, int x, int y, int depth)
 {
-  const CtxT<Pix> &c = *e.c;
+  CtuST<Pix> *S = e.S = sm(e.S);
+  uint8_t *ctx = S->tmp.ctx;
   const CuRec *cur_cu = tcu(e, x, y);
   const int cu_width = 64 >> depth;
-  if (depth == 3) enc_bin(&c.S->tb, e.cs->ctx, CTX_PART_SIZE, cur_cu->part_size == SIZE_2Nx2N ? 1 : 0);
+  if (depth == 3) enc_bin(&S->tb, ctx, CTX_PART_SIZE, cur_cu->part_size == SIZE_2Nx2N ? 1 : 0);
   const int num_pu = cur_cu->part_size == SIZE_NxN ? 4 : 1;
-  int flag[4];
+  unsigned flag = 0;                // bit j: PU j's mode is an MPM
   int mode0 = 0;
   for (int j = 0; j < num_pu; ++j) {
     const int pw = cu_width / 2;
@@ -606,24 +616,27 @@ template <typename Pix> CTU_FN_NOINLINE void enc_coding_unit(const EncTrack<Pix>
     int8_t preds[3];
     intra_mpm(pu_y, left_pu, above_pu, preds);
     if (j == 0) mode0 = cur_pu->mode;
-    flag[j] = cur_pu->mode == preds[0] || cur_pu->mode == preds[1] || cur_pu->mode == preds[2];
+    if (cur_pu->mode == preds[0] || cur_pu->mode == preds[1] || cur_pu->mode == preds[2]) flag |= 1u << j;
   }
-  for (int j = 0; j < num_pu; ++j) enc_bin(&c.S->tb, e.cs->ctx, CTX_INTRA_MODE, flag[j]);
-  enc_bin(&c.S->tb, e.cs->ctx, CTX_CHROMA_PRED, cur_cu->mode_chroma == mode0 ? 0 : 1);
+  for (int j = 0; j < num_pu; ++j) enc_bin(&S->tb, ctx, CTX_INTRA_MODE, (flag >> j) & 1);
+  enc_bin(&S->tb, ctx, CTX_CHROMA_PRED, cur_cu->mode_chroma == mode0 ? 0 : 1);
   enc_transform_tree(e, x, y, depth);
 }
 
 // kvz_encode_coding_tree: explicit traversal of the CU quadtree in coding order
-template <typename Pix> CTU_FN_NOINLINE void enc_coding_tree(const EncTrack<Pix> &e, int x0, int y0)
+template <typename Pix> CTU_FN_NOINLINE void enc_coding_tree(EncTrack<Pix> e)
 {
-  const CtxT<Pix> &c = *e.c;
-  const int Wd = c.cfg->width, H = c.cfg->height;
-  // depth-first with a small stack of (x, y, depth)
-  int sx[16], sy[16], sd[16], sp = 0;
-  sx[0] = x0; sy[0] = y0; sd[0] = 0; sp = 1;
+  CtuST<Pix> *S = e.S = sm(e.S);
+  const int Wd = S->cfg.width, H = S->cfg.height;
+  // depth-first with a small stack of (x - x0) << 16 | (y - y0) << 8 | depth, at most 13 entries deep; it lives in the
+  // rough search's SATD table, idle after the search
+  int32_t *stk = S->satd;
+  int sp = 1;
+  stk[0] = 0;
   while (sp > 0) {
     --sp;
-    const int x = sx[sp], y = sy[sp], depth = sd[sp];
+    const int v = stk[sp];
+    const int x = e.x0 + (v >> 16), y = e.y0 + ((v >> 8) & 0xff), depth = v & 0xff;
     const CuRec *cur_cu = tcu(e, x, y);
     const int cu_width = 64 >> depth, half = cu_width >> 1;
     const int split_flag = cur_cu->depth > depth;
@@ -635,14 +648,15 @@ template <typename Pix> CTU_FN_NOINLINE void enc_coding_tree(const EncTrack<Pix>
         int split_model = 0;
         if (x > 0 && tcu(e, x - 1, y)->depth > depth) ++split_model;
         if (y > 0 && tcu(e, x, y - 1)->depth > depth) ++split_model;
-        enc_bin(&c.S->tb, e.cs->ctx, CTX_SPLIT + split_model, split_flag);
+        enc_bin(&S->tb, S->tmp.ctx, CTX_SPLIT + split_model, split_flag);
       }
       if (split_flag || border) {
         // push in reverse so that the children pop in z-order
-        if (!border || (border_split_x && border_split_y)) { sx[sp] = x + half; sy[sp] = y + half; sd[sp] = depth + 1; ++sp; }
-        if (!border_y || border_split_y) { sx[sp] = x; sy[sp] = y + half; sd[sp] = depth + 1; ++sp; }
-        if (!border_x || border_split_x) { sx[sp] = x + half; sy[sp] = y; sd[sp] = depth + 1; ++sp; }
-        sx[sp] = x; sy[sp] = y; sd[sp] = depth + 1; ++sp;
+        const int c = v + 1;          // (x, y, depth + 1)
+        if (!border || (border_split_x && border_split_y)) stk[sp++] = c + (half << 16) + (half << 8);
+        if (!border_y || border_split_y) stk[sp++] = c + (half << 8);
+        if (!border_x || border_split_x) stk[sp++] = c + (half << 16);
+        stk[sp++] = c;
         continue;
       }
     }
@@ -652,47 +666,55 @@ template <typename Pix> CTU_FN_NOINLINE void enc_coding_tree(const EncTrack<Pix>
 
 // The CTU's effect on the real coder's models; afterwards the row's state is published (and handed to the next row
 // after the second CTU: WPP, encoderstate.c:759-771).  Leader only inside.
-template <typename Pix> CTU_FN_NOINLINE void ctu_track_models(const CtxT<Pix> &c, const FrameDevT<Pix> *F, int cx, int cy)
+template <typename Pix> CTU_FN_NOINLINE void ctu_track_models(CtuST<Pix> *S, const FrameDevT<Pix> *F, int cx, int cy)
 {
+  S = sm(S);
   CTU_LEADER {
     // the models are walked in the search's spare copy (shared memory; the search is over): cost walks that adapt
     // them read and write shared memory, not the leader's stack
-    CabacState &cs = c.S->tmp;
-    cs = c.S->cabac0;
+    CabacState &cs = S->tmp;
+    cs = S->cabac0;
     cs.update = 1;
-    if (c.cfg->sao_type) {
+    if (S->cfg.sao_type) {
       const SaoRec *sl = &F->sao[2 * (cy * F->wlcu + cx)], *sc = sl + 1;
-      if (cx > 0) enc_bin(&c.S->tb, cs.ctx, CTX_SAO_MERGE, sl->merge_left_flag);
-      if (cy > 0 && !sl->merge_left_flag) enc_bin(&c.S->tb, cs.ctx, CTX_SAO_MERGE, sl->merge_up_flag);
+      if (cx > 0) enc_bin(&S->tb, cs.ctx, CTX_SAO_MERGE, sl->merge_left_flag);
+      if (cy > 0 && !sl->merge_left_flag) enc_bin(&S->tb, cs.ctx, CTX_SAO_MERGE, sl->merge_up_flag);
       if (!sl->merge_left_flag && !sl->merge_up_flag) {
-        enc_bin(&c.S->tb, cs.ctx, CTX_SAO_TYPE, sl->type != 0);
-        enc_bin(&c.S->tb, cs.ctx, CTX_SAO_TYPE, sc->type != 0);
+        enc_bin(&S->tb, cs.ctx, CTX_SAO_TYPE, sl->type != 0);
+        enc_bin(&S->tb, cs.ctx, CTX_SAO_TYPE, sc->type != 0);
       }
     }
-    EncTrack<Pix> e = { &c, &c.S->lv[0], cx * 64, cy * 64, &cs };
-    enc_coding_tree(e, cx * 64, cy * 64);
+    const EncTrack<Pix> e = { S, cx * 64, cy * 64 };
+    enc_coding_tree(e);
     cs.update = 0;
     F->row_ctx[cy] = cs;
-    if (c.cfg->wpp && cx == 1 && cy + 1 < F->hlcu) F->row_ctx[cy + 1] = cs;
+    if (S->cfg.wpp && cx == 1 && cy + 1 < F->hlcu) F->row_ctx[cy + 1] = cs;
   }
   CTU_SYNC();
 }
 
 // ------------------------------------------------------------------------------------------------ whole CTU job
+// The per-CTU functions find the configuration, the work area and the tables in the shared state block: they are
+// copied there first.
 template <typename Pix> CTU_FN void ctu_job(const CtxT<Pix> &c, const FrameDevT<Pix> *F, SaoStats *sao_scratch, int cx, int cy)
 {
-  { PROF_T0(PR_LOAD); ctu_load(c, F, cx, cy); PROF_ADD(c.S, PR_LOAD); }
-  { PROF_T0(PR_SEARCH); search_ctu(c, cx * 64, cy * 64); PROF_ADD(c.S, PR_SEARCH); }
+  CtuST<Pix> *S = sm(c.S);
+  #pragma unroll 1
+  for (int i = CTU_TID; i < (int)(sizeof(CtuConfig) / 4); i += CTU_NT) ((uint32_t *)&S->cfg)[i] = ((const uint32_t *)c.cfg)[i];
+  CTU_LEADER S->W = c.W;
+  CTU_SYNC();
+  { PROF_T0(PR_LOAD); ctu_load(S, F, cx, cy); PROF_ADD(S, PR_LOAD); }
+  { PROF_T0(PR_SEARCH); sm_tables_load(&S->tb, c.T); search_ctu(S, cx * 64, cy * 64); PROF_ADD(S, PR_SEARCH); }
   PROF_T0(PR_STORE);
-  ctu_store(c, F, cx, cy);
+  ctu_store(S, F, cx, cy);
 #if defined(__CUDA_ARCH__)
   __threadfence();
 #endif
   CTU_SYNC();
-  PROF_ADD(c.S, PR_STORE);
-  if (c.cfg->deblock_enable) { PROF_T0(PR_DEBLOCK); ctu_deblock(c, F, cx, cy); PROF_ADD(c.S, PR_DEBLOCK); }
-  if (c.cfg->sao_type) { PROF_T0(PR_SAO); ctu_sao_search(c, F, sao_scratch, cx, cy); PROF_ADD(c.S, PR_SAO); }
-  { PROF_T0(PR_TRACK); ctu_track_models(c, F, cx, cy); PROF_ADD(c.S, PR_TRACK); }
+  PROF_ADD(S, PR_STORE);
+  if (S->cfg.deblock_enable) { PROF_T0(PR_DEBLOCK); ctu_deblock(S, F, cx, cy); PROF_ADD(S, PR_DEBLOCK); }
+  if (S->cfg.sao_type) { PROF_T0(PR_SAO); ctu_sao_search(S, F, sao_scratch, cx, cy); PROF_ADD(S, PR_SAO); }
+  { PROF_T0(PR_TRACK); ctu_track_models(S, F, cx, cy); PROF_ADD(S, PR_TRACK); }
 }
 
 // ------------------------------------------------------------------------------------------------ SAO application

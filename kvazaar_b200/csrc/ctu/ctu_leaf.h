@@ -477,10 +477,11 @@ CTU_FN void rough_diff_block(const IntraRefs<Pix> *r, const RoughExt<Pix> *ext, 
 }
 
 // SATD (satd_NxN) and, for 4x4, SAD of the prediction of every mode against the source block.
-// satd_out / sad_out: [35] ints.  `ext`: scratch (the arena: no transform-unit job is running during the rough search).
+// satd_out / sad_out: [35] ints.  Everything but `src` is in shared memory.  `ext`: scratch (the arena: no transform-unit job is running during the rough search).
 template <typename Pix> CTU_FN_NOINLINE void rough_costs_all_modes(const IntraRefs<Pix> *r, RoughExt<Pix> *ext, int log2w, int color, const Pix *src, int src_stride,
                                   int32_t *satd_out, int32_t *sad_out, bool want_sad)
 {
+  r = sm(r); ext = sm(ext); satd_out = sm(satd_out); sad_out = sm(sad_out);
   const int w = 1 << log2w;
   #pragma unroll 1
   for (int m = CTU_TID; m < 35; m += CTU_NT) { satd_out[m] = 0; sad_out[m] = 0; }

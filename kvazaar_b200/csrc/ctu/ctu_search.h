@@ -46,6 +46,8 @@ template <typename Pix> struct CtuST {                       // per-CTA scalar s
   CabacState cabac0;                // state->cabac: the real coder's models when the CTU starts (constant)
   CabacState sc;                    // state->search_cabac
   CabacState tmp;                   // temp_cabac of the combined-CU path (search.c:989); after the search: ctu_track_models' models
+  CtuConfig cfg;                    // the picture's configuration and this CTA's work area, set by ctu_job: the per-CTU
+  CtuWorkT<Pix> *W;                 //   functions read them here (LDS) instead of through the caller's context
   SearchFrame fr[5];
   double ret_cost;
   IntraRefs<Pix> refs[3];
@@ -78,6 +80,8 @@ template <typename Pix> struct CtuST {                       // per-CTA scalar s
 };
 using CtuS = CtuST<uint8_t>;          // (8-bit alias, see CtuWork)
 
+// What the CTU job is started with (ctu_job).  The functions below it take the shared state block instead and re-derive
+// it with sm(): a context passed by reference would live on the caller's stack, and its pointers would be generic.
 template <typename Pix> struct CtxT {
   const CtuTables *T;
   const CtuConfig *cfg;
@@ -103,20 +107,20 @@ CTU_FN void intra_mpm(int y, const CuRec *left, const CuRec *above, int8_t *pred
   }
 }
 // kvz_luma_mode_bits (ref: search_intra.c:641-679); leader only
-template <typename Pix> CTU_FN double luma_mode_bits(const CtxT<Pix> &c, int mode, const int8_t *preds)
+template <typename Pix> CTU_FN double luma_mode_bits(CtuST<Pix> *S, int mode, const int8_t *preds)
 {
   double bits = 0;
   const bool in = mode == preds[0] || mode == preds[1] || mode == preds[2];
-  cabac_bin(&c.S->tb, &c.S->sc, CTX_INTRA_MODE, in, &bits);
+  cabac_bin(&S->tb, &S->sc, CTX_INTRA_MODE, in, &bits);
   if (in) bits += (mode == preds[0]) ? 1 : 2;
   else bits += 5;
   return bits;
 }
 // kvz_chroma_mode_bits (ref: search_intra.c:682-701); leader only
-template <typename Pix> CTU_FN double chroma_mode_bits(const CtxT<Pix> &c, int chroma_mode, int luma_mode)
+template <typename Pix> CTU_FN double chroma_mode_bits(CtuST<Pix> *S, int chroma_mode, int luma_mode)
 {
   double bits = 0;
-  cabac_bin(&c.S->tb, &c.S->sc, CTX_CHROMA_PRED, chroma_mode != luma_mode, &bits);
+  cabac_bin(&S->tb, &S->sc, CTX_CHROMA_PRED, chroma_mode != luma_mode, &bits);
   if (chroma_mode != luma_mode) bits += 2.0;
   return bits;
 }
@@ -155,30 +159,33 @@ template <typename Pix> CTU_FN void copy_cu_coeffs(LcuLevel<Pix> *from, LcuLevel
   #pragma unroll 1
   for (int e = CTU_TID; e < wc * wc; e += CTU_NT) { to->coeff_u[zc + e] = from->coeff_u[zc + e]; to->coeff_v[zc + e] = from->coeff_v[zc + e]; }
 }
-template <typename Pix> CTU_FN_NOINLINE void work_tree_copy_up(const CtxT<Pix> &c, int xl, int yl, int depth)
+template <typename Pix> CTU_FN_NOINLINE void work_tree_copy_up(CtuST<Pix> *S, int xl, int yl, int depth)
 {
+  S = sm(S);
   const int w = 64 >> depth;
   PROF_T0(PR_COPY);
-  copy_cu_info(&c.S->lv[depth + 1], &c.S->lv[depth], xl, yl, w);
-  copy_cu_pixels(&c.S->lv[depth + 1], &c.S->lv[depth], xl, yl, w);
-  copy_cu_coeffs(&c.S->lv[depth + 1], &c.S->lv[depth], xl, yl, w);
+  copy_cu_info(&S->lv[depth + 1], &S->lv[depth], xl, yl, w);
+  copy_cu_pixels(&S->lv[depth + 1], &S->lv[depth], xl, yl, w);
+  copy_cu_coeffs(&S->lv[depth + 1], &S->lv[depth], xl, yl, w);
   CTU_SYNC();
-  PROF_ADD(c.S, PR_COPY);
+  PROF_ADD(S, PR_COPY);
 }
-template <typename Pix> CTU_FN_NOINLINE void work_tree_copy_down(const CtxT<Pix> &c, int xl, int yl, int depth)
+template <typename Pix> CTU_FN_NOINLINE void work_tree_copy_down(CtuST<Pix> *S, int xl, int yl, int depth)
 {
+  S = sm(S);
   const int w = 64 >> depth;
   PROF_T0(PR_COPY);
   for (int i = depth + 1; i <= 4; ++i) {
-    copy_cu_info(&c.S->lv[depth], &c.S->lv[i], xl, yl, w);
-    copy_cu_pixels(&c.S->lv[depth], &c.S->lv[i], xl, yl, w);
+    copy_cu_info(&S->lv[depth], &S->lv[i], xl, yl, w);
+    copy_cu_pixels(&S->lv[depth], &S->lv[i], xl, yl, w);
   }
   CTU_SYNC();
-  PROF_ADD(c.S, PR_COPY);
+  PROF_ADD(S, PR_COPY);
 }
 // kvz_lcu_fill_trdepth
 template <typename Pix> CTU_FN_NOINLINE void fill_trdepth(LcuLevel<Pix> *L, int xl, int yl, int depth, int tr_depth)
 {
+  L = sm(L);
   const int n = (64 >> depth) >> 2;
   #pragma unroll 1
   for (int e = CTU_TID; e < n * n; e += CTU_NT) cu_at(L, xl + 4 * (e % n), yl + 4 * (e / n))->tr_depth = (uint8_t)tr_depth;
@@ -187,7 +194,8 @@ template <typename Pix> CTU_FN_NOINLINE void fill_trdepth(LcuLevel<Pix> *L, int 
 // lcu_fill_cu_info (intra fields only); `cu` may alias one of the targets
 template <typename Pix> CTU_FN_NOINLINE void fill_cu_info(LcuLevel<Pix> *L, int xl, int yl, int width, const CuRec *cu)
 {
-  const CuRec v = *cu;
+  L = sm(L);
+  const CuRec v = *sm(cu);
   CTU_SYNC();
   const int n = width >> 2;
   #pragma unroll 1
@@ -203,19 +211,19 @@ template <typename Pix> CTU_FN_NOINLINE void fill_cu_info(LcuLevel<Pix> *L, int 
 CTU_FN int tu_log2(int depth, int color) { return color == 0 ? 6 - depth : (depth < 4 ? 5 - depth : 2); }
 CTU_FN int stage_key_of(int xl, int yl, int depth) { return (xl << 16) | (yl << 8) | depth; }
 // coefficients of the unit of `color` at (xl, yl, depth) on level L: the staged copy when it is this unit's
-template <typename Pix> CTU_FN const int16_t *unit_coeffs(const CtxT<Pix> &c, LcuLevel<Pix> *L, int color, int xl, int yl, int depth, uint64_t *mask)
+template <typename Pix> CTU_FN const int16_t *unit_coeffs(CtuST<Pix> *S, LcuLevel<Pix> *L, int color, int xl, int yl, int depth, uint64_t *mask)
 {
   *mask = COEFF_NO_MASK;
-  if (c.S->stage_key[color] == stage_key_of(xl, yl, depth)) { *mask = c.S->stage_mask[color]; return color == 0 ? c.S->stage_y : c.S->stage_c[color - 1]; }
+  if (S->stage_key[color] == stage_key_of(xl, yl, depth)) { *mask = S->stage_mask[color]; return color == 0 ? S->stage_y : S->stage_c[color - 1]; }
   if (color == 0) return &L->coeff_y[zorder(64, xl, yl)];
   return (color == 1 ? L->coeff_u : L->coeff_v) + zorder(32, xl >> 1, yl >> 1);
 }
 
-template <typename Pix> CTU_FN double coeff_cost_of_unit(const CtxT<Pix> &c, CabacState *sc, LcuLevel<Pix> *L, int color, int xl, int yl, int depth, int log2n, int type, int scan)
+template <typename Pix> CTU_FN double coeff_cost_of_unit(CtuST<Pix> *S, CabacState *sc, LcuLevel<Pix> *L, int color, int xl, int yl, int depth, int log2n, int type, int scan)
 {
   uint64_t mask;
-  const int16_t *co = unit_coeffs(c, L, color, xl, yl, depth, &mask);
-  return coeff_cost_serial(&c.S->tb, &c.S->tb, c.cfg, sc, co, log2n, type, scan, 0, mask);
+  const int16_t *co = unit_coeffs(S, L, color, xl, yl, depth, &mask);
+  return coeff_cost_serial(&S->tb, &S->tb, &S->cfg, sc, co, log2n, type, scan, 0, mask);
 }
 
 // The class of a transform-unit task for for_tu_tasks: its unit's log2 side (bits 0..2) and luma or chroma.
@@ -230,7 +238,7 @@ CTU_FN int tu_class(int log2n, int color) { return log2n | (color ? 8 : 0); }
 // -- go to the warps in turn.  (Half-warp teams for the 4x4 and 8x8 units of mixed batches were measured slower: the
 // two halves' serial sections -- RDOQ's walk, the coefficient bits -- diverge and run one after the other, so a pair
 // takes about as long as two units on whole warps.)  f(team, slot base, task) must synchronise with tsync(team) only.
-template <typename Pix, class K, class F> CTU_FN void for_tu_tasks(const CtxT<Pix> &c, int ntasks, K class_of, F f)
+template <typename Pix, class K, class F> CTU_FN void for_tu_tasks(CtuST<Pix> *S, int ntasks, K class_of, F f)
 {
   CTU_SYNC();
   const int nw = CTU_NWARPS;
@@ -259,10 +267,10 @@ template <typename Pix, class K, class F> CTU_FN void for_tu_tasks(const CtxT<Pi
   }
   if (cta) {
     const Team tm = team_cta();
-    for (int t = 0; t < ntasks; ++t) if ((cta >> t) & 1) f(tm, c.S->arena, t);
+    for (int t = 0; t < ntasks; ++t) if ((cta >> t) & 1) f(tm, S->arena, t);
     CTU_SYNC();
   }
-  unsigned char *base = c.S->arena + (size_t)CTU_WARP * warp_bytes;
+  unsigned char *base = S->arena + (size_t)CTU_WARP * warp_bytes;
   if (whole) {
     const Team tm = team_warp();
     for (int t = 0; t < ntasks; ++t) if ((whole >> t) & 1) f(tm, base, t);
@@ -274,15 +282,16 @@ template <typename Pix, class K, class F> CTU_FN void for_tu_tasks(const CtxT<Pi
   }
   CTU_SYNC();
 }
+template <typename Pix, class K, class F> CTU_FN void for_tu_tasks(const CtxT<Pix> &c, int ntasks, K class_of, F f) { for_tu_tasks(sm(c.S), ntasks, class_of, f); }
 
 template <typename Pix> CTU_FN TuS<Pix> tu_at(unsigned char *slot, int nn) { TuS<Pix> t; t.base = slot; t.nn = nn; t.ncg = nn >= 16 ? nn / 16 : 1; return t; }
 
 // leaf part of kvz_intra_recon_cu + kvz_quantize_lcu_residual (ref: intra.c:676-696, transform.c:448-508): the
 // colours of the leaf are independent jobs (prediction only reads neighbours outside the unit).
 // refs_valid: bit per colour whose S->refs[] already hold this unit's references.
-template <typename Pix> CTU_FN_NOINLINE void intra_recon_leaf(const CtxT<Pix> &c, LcuLevel<Pix> *L, int x, int y, int depth, int mode_luma, int mode_chroma, CuRec *cur_cu, int leaf, int refs_valid)
+template <typename Pix> CTU_FN_NOINLINE void intra_recon_leaf(CtuST<Pix> *S, LcuLevel<Pix> *L, int x, int y, int depth, int mode_luma, int mode_chroma, CuRec *cur_cu, int leaf, int refs_valid)
 {
-  CtuST<Pix> *S = c.S;
+  S = sm(S); L = sm(L); cur_cu = sm(cur_cu);
   const int xl = x & 63, yl = y & 63;
   CuRec *cur_tu = cu_at(L, xl, yl);
   const bool has_luma = mode_luma != -1;
@@ -293,18 +302,18 @@ template <typename Pix> CTU_FN_NOINLINE void intra_recon_leaf(const CtxT<Pix> &c
   {
     int need = 0;
     for (int col = first; col <= last; ++col) if (!((refs_valid >> col) & 1)) need |= 1 << col;
-    if (need) build_refs_multi(&c.S->tb, c.cfg->width, c.cfg->height, c.W, L, pack_log2w(tu_log2(depth, 0), tu_log2(depth, 1), tu_log2(depth, 2)), need, x, y, S->refs);
+    if (need) build_refs_multi(&S->tb, S->cfg.width, S->cfg.height, S->W, L, pack_log2w(tu_log2(depth, 0), tu_log2(depth, 1), tu_log2(depth, 2)), need, x, y, S->refs);
   }
   PROF_ADD(S, PR_REFS);
   // cur_pu of quantize_tr_residual: the RDOQ context selector reads its depths before the cbf bits change
   const int rdoq_tr_depth = (int)cur_cu->tr_depth - (int)cur_cu->depth + (cur_cu->part_size == SIZE_NxN ? 1 : 0);
   PROF_T0(PR_QRES4);
   // tasks luma, U, V: U and V share a warp when their units are 4x4
-  for_tu_tasks(c, last - first + 1, [&](int t) { return tu_class(tu_log2(depth, first + t), first + t); }, [&](const Team &tm, unsigned char *slot, int t) {
+  for_tu_tasks(S, last - first + 1, [&](int t) { return tu_class(tu_log2(depth, first + t), first + t); }, [&](const Team &tm, unsigned char *slot, int t) {
     const int col = first + t;
     const int log2n = tu_log2(depth, col), n = 1 << log2n;
     const TuS<Pix> tu = tu_at<Pix>(slot, n * n);
-    const Plane<Pix> P = plane_of(c.W, L, col);
+    const Plane<Pix> P = plane_of(S->W, L, col);
     const int sh = col ? 1 : 0;
     const int off = (xl >> sh) + (yl >> sh) * P.lw;
     const int mode = col == 0 ? mode_luma : mode_chroma;
@@ -312,7 +321,7 @@ template <typename Pix> CTU_FN_NOINLINE void intra_recon_leaf(const CtxT<Pix> &c
     // the chroma mode search predicts with its candidate while the record still holds the luma mode (bits 8.. of refs_valid)
     const int scan_mode = (col != 0 && (refs_valid >> 8)) ? (refs_valid >> 8) - 1 : mode;
     TuJob<Pix> j = { &S->refs[col], P.src + off, P.lw, col, log2n, mode, scan_order_intra(scan_mode, depth), rdoq_tr_depth };
-    const int ts = tu_eval(tm, &c.S->tb, &S->tb, c.cfg, S->cabac0.ctx, &S->sc, tu, j);
+    const int ts = tu_eval(tm, &S->tb, &S->tb, &S->cfg, S->cabac0.ctx, &S->sc, tu, j);
     // write back: reconstruction and coefficients of the level, staged copy for the cost functions
     Pix *rec = P.rec + off;
     int16_t *co = P.coeff + zorder(P.lw, xl >> sh, yl >> sh);
@@ -335,7 +344,7 @@ template <typename Pix> CTU_FN_NOINLINE void intra_recon_leaf(const CtxT<Pix> &c
   });
   PROF_ADD_AS(S, PR_QRES4, pr_qres_of(tu_log2(depth, first)));
   CTU_LEADER {
-    const bool ts_branch = depth == 4 && c.cfg->trskip_enable;       // 4x4 luma units only (transform.c:366)
+    const bool ts_branch = depth == 4 && S->cfg.trskip_enable;       // 4x4 luma units only (transform.c:366)
     for (int col = first; col <= last; ++col) {
       cbf_clear(&cur_cu->cbf, depth, col);
       if (S->res[0][col].has) cbf_set(&cur_cu->cbf, depth, col);
@@ -349,16 +358,17 @@ template <typename Pix> CTU_FN_NOINLINE void intra_recon_leaf(const CtxT<Pix> &c
 
 // kvz_intra_recon_cu (ref: intra.c:623-698).  cur_cu == NULL: the CU record of the level at (x, y).  Leaves the SSDs
 // of the reconstructed colours in S->ssd[leaf][colour] (0 for the colours not touched).
-template <typename Pix> CTU_FN_NOINLINE void intra_recon_cu(const CtxT<Pix> &c, LcuLevel<Pix> *L, int x, int y, int depth, int mode_luma, int mode_chroma, CuRec *cur_cu, int refs_valid)
+template <typename Pix> CTU_FN_NOINLINE void intra_recon_cu(CtuST<Pix> *S, LcuLevel<Pix> *L, int x, int y, int depth, int mode_luma, int mode_chroma, CuRec *cur_cu, int refs_valid)
 {
+  S = sm(S); L = sm(L);
   const int xl = x & 63, yl = y & 63;
-  if (cur_cu == NULL) cur_cu = cu_at(L, xl, yl);
+  cur_cu = cur_cu == NULL ? cu_at(L, xl, yl) : sm(cur_cu);
   CTU_LEADER {
     if (mode_luma >= 0) cbf_clear(&cur_cu->cbf, depth, 0);
     if (mode_chroma >= 0) { cbf_clear(&cur_cu->cbf, depth, 1); cbf_clear(&cur_cu->cbf, depth, 2); }
     for (int k = 0; k < 4; ++k) {
-      if (mode_luma >= 0) c.S->ssd[k][0] = 0;
-      if (mode_chroma >= 0) { c.S->ssd[k][1] = 0; c.S->ssd[k][2] = 0; }
+      if (mode_luma >= 0) S->ssd[k][0] = 0;
+      if (mode_chroma >= 0) { S->ssd[k][1] = 0; S->ssd[k][2] = 0; }
     }
   }
   CTU_SYNC();
@@ -373,7 +383,7 @@ template <typename Pix> CTU_FN_NOINLINE void intra_recon_cu(const CtxT<Pix> &c, 
         if (mode_chroma >= 0) { cbf_clear(&child->cbf, depth + 1, 1); cbf_clear(&child->cbf, depth + 1, 2); }
       }
       CTU_SYNC();
-      intra_recon_leaf(c, L, cx, cy, depth + 1, mode_luma, mode_chroma, child, k, refs_valid & ~0xFF);
+      intra_recon_leaf(S, L, cx, cy, depth + 1, mode_luma, mode_chroma, child, k, refs_valid & ~0xFF);
     }
     CTU_LEADER {
       const uint16_t child_cbfs[3] = { cu_at(L, xl + offset, yl)->cbf, cu_at(L, xl, yl + offset)->cbf, cu_at(L, xl + offset, yl + offset)->cbf };
@@ -382,7 +392,7 @@ template <typename Pix> CTU_FN_NOINLINE void intra_recon_cu(const CtxT<Pix> &c, 
     }
     CTU_SYNC();
   } else {
-    intra_recon_leaf(c, L, x, y, depth, mode_luma, mode_chroma, cur_cu, 0, refs_valid);
+    intra_recon_leaf(S, L, x, y, depth, mode_luma, mode_chroma, cur_cu, 0, refs_valid);
   }
 }
 
@@ -392,21 +402,21 @@ template <typename Pix> CTU_FN_NOINLINE void intra_recon_cu(const CtxT<Pix> &c, 
 // models.  Except chroma at depth 4, which is reconstructed again: the candidate quantised it with the cbf context of
 // tr_depth 1 (pred_cu of search_intra_rdo), the CU's reconstruction uses its record's tr_depth 4 - depth 3 + NxN = 2
 // (rdo.c:919).
-template <typename Pix> CTU_FN_NOINLINE void write_back_candidate(const CtxT<Pix> &c, LcuLevel<Pix> *L, int x, int y, int depth, int mode, bool with_chroma)
+template <typename Pix> CTU_FN_NOINLINE void write_back_candidate(CtuST<Pix> *S, LcuLevel<Pix> *L, int x, int y, int depth, int mode, bool with_chroma)
 {
-  CtuST<Pix> *S = c.S;
+  S = sm(S); L = sm(L);
   const int xl = x & 63, yl = y & 63;
   const int last = with_chroma && depth < 4 ? 2 : 0;
   PROF_T0(PR_WRITEBACK);
   int cand = 0;
   while (S->cand_modes[cand] != mode) ++cand;
-  const bool ts_split = depth == 4 && c.cfg->trskip_enable;
+  const bool ts_split = depth == 4 && S->cfg.trskip_enable;
   for (int col = 0; col <= last; ++col) {
     const int log2n = tu_log2(depth, col), n = 1 << log2n;
     const int unit = col == 0 ? (ts_split ? 2 * cand + S->res[cand][0].tr_skip : cand) : cand;
-    const Pix *kr = (col == 0 ? c.W->cand.rec_y : c.W->cand.rec_c[col - 1]) + unit * n * n;
-    const int16_t *kq = (col == 0 ? c.W->cand.q_y : c.W->cand.q_c[col - 1]) + unit * n * n;
-    const Plane<Pix> P = plane_of(c.W, L, col);
+    const Pix *kr = (col == 0 ? S->W->cand.rec_y : S->W->cand.rec_c[col - 1]) + unit * n * n;
+    const int16_t *kq = (col == 0 ? S->W->cand.q_y : S->W->cand.q_c[col - 1]) + unit * n * n;
+    const Plane<Pix> P = plane_of(S->W, L, col);
     const int sh = col ? 1 : 0;
     Pix *rec = P.rec + (xl >> sh) + (yl >> sh) * P.lw;
     int16_t *co = P.coeff + zorder(P.lw, xl >> sh, yl >> sh);
@@ -433,15 +443,18 @@ template <typename Pix> CTU_FN_NOINLINE void write_back_candidate(const CtxT<Pix
   }
   CTU_SYNC();
   PROF_ADD(S, PR_WRITEBACK);
-  if (with_chroma && depth == 4) intra_recon_cu(c, L, x, y, depth, -1, mode, NULL, 7);
+  if (with_chroma && depth == 4) intra_recon_cu(S, L, x, y, depth, -1, mode, NULL, 7);
 }
 
 // ------------------------------------------------------------------------------------------------ RD costs
 // kvz_cu_rd_cost_luma for a leaf (tr_depth == depth), the search models not adapting (update == 0: the candidates of
-// search_intra_rdo).  Leader only.  ssd / coeff_bits: the unit's SSD and kvz_get_coeff_cost (0 when cbf is clear).
-template <typename Pix> CTU_FN_NOINLINE double cu_rd_cost_luma_leaf(const CtxT<Pix> &c, LcuLevel<Pix> *L, int xl, int yl, int depth, const CuRec *pred_cu, int ssd, double coeff_bits_y)
+// search_intra_rdo; the temporary CU is S->pred_cu).  Leader only.  ssd / coeff_bits: the unit's SSD and
+// kvz_get_coeff_cost (0 when cbf is clear).
+template <typename Pix> CTU_FN_NOINLINE double cu_rd_cost_luma_leaf(CtuST<Pix> *S, LcuLevel<Pix> *L, int xl, int yl, int depth, int ssd, double coeff_bits_y)
 {
-  CabacState *sc = &c.S->sc;
+  S = sm(S); L = sm(L);
+  const CuRec *pred_cu = &S->pred_cu;
+  CabacState *sc = &S->sc;
   const int width = 64 >> depth;
   CuRec *tr_cu = cu_at(L, xl, yl);
   double coeff_bits = 0, tr_tree_bits = 0;
@@ -449,24 +462,25 @@ template <typename Pix> CTU_FN_NOINLINE double cu_rd_cost_luma_leaf(const CtxT<P
   const bool intra_split_flag = pred_cu->part_size == SIZE_NxN && depth == 3;
   const int max_tr_depth = 0 + (intra_split_flag ? 1 : 0);
   if (width <= 32 && width > 4 && !intra_split_flag && imin((int)tr_cu->tr_depth, depth) - (int)tr_cu->depth < max_tr_depth)
-    cabac_bin(&c.S->tb, sc, CTX_TRANS_SUBDIV + (5 - (6 - depth)), tr_depth > 0, &tr_tree_bits);
+    cabac_bin(&S->tb, sc, CTX_TRANS_SUBDIV + (5 - (6 - depth)), tr_depth > 0, &tr_tree_bits);
   if (sc->update && tr_cu->tr_depth == tr_cu->depth) {
     const int off = CTX_CBF_CHROMA + (depth - (int)tr_cu->depth);
-    cabac_bin(&c.S->tb, sc, off, cbf_is_set(tr_cu->cbf, depth, 1), &tr_tree_bits);
-    cabac_bin(&c.S->tb, sc, off, cbf_is_set(tr_cu->cbf, depth, 2), &tr_tree_bits);
+    cabac_bin(&S->tb, sc, off, cbf_is_set(tr_cu->cbf, depth, 1), &tr_tree_bits);
+    cabac_bin(&S->tb, sc, off, cbf_is_set(tr_cu->cbf, depth, 2), &tr_tree_bits);
   }
   const int is_tr_split = (int)tr_cu->tr_depth - (int)tr_cu->depth;
   const int is_set = cbf_is_set(tr_cu->cbf, depth, 0);
-  cabac_bin(&c.S->tb, sc, CTX_CBF_LUMA + (is_tr_split ? 0 : 1), is_set, &tr_tree_bits);     // pred_cu->type == CU_INTRA
+  cabac_bin(&S->tb, sc, CTX_CBF_LUMA + (is_tr_split ? 0 : 1), is_set, &tr_tree_bits);     // pred_cu->type == CU_INTRA
   if (is_set) coeff_bits += coeff_bits_y;
   const double bits = tr_tree_bits + coeff_bits;
-  return (double)ssd * 0.8 + bits * c.cfg->lambda;
+  return (double)ssd * 0.8 + bits * S->cfg.lambda;
 }
 
 // kvz_cu_rd_cost_chroma for a leaf, update == 0.  Leader only.
-template <typename Pix> CTU_FN_NOINLINE double cu_rd_cost_chroma_leaf(const CtxT<Pix> &c, LcuLevel<Pix> *L, int xl, int yl, int depth, const CuRec *pred_cu, int ssd, double coeff_bits_u, double coeff_bits_v)
+template <typename Pix> CTU_FN_NOINLINE double cu_rd_cost_chroma_leaf(CtuST<Pix> *S, LcuLevel<Pix> *L, int xl, int yl, int depth, const CuRec *pred_cu, int ssd, double coeff_bits_u, double coeff_bits_v)
 {
-  CabacState *sc = &c.S->sc;
+  S = sm(S); L = sm(L); pred_cu = sm(pred_cu);
+  CabacState *sc = &S->sc;
   CuRec *tr_cu = cu_at(L, xl, yl);
   double tr_tree_bits = 0, coeff_bits = 0;
   if (xl % 8 != 0 || yl % 8 != 0) return 0;
@@ -474,33 +488,35 @@ template <typename Pix> CTU_FN_NOINLINE double cu_rd_cost_chroma_leaf(const CtxT
   if (depth < 4 && (!sc->update || tr_cu->tr_depth != tr_cu->depth)) {
     const int tr_depth = depth - (int)pred_cu->depth;
     const int off = CTX_CBF_CHROMA + tr_depth;
-    if (tr_depth == 0 || cbf_is_set(tr_cu->cbf, depth - 1, 1)) cabac_bin(&c.S->tb, sc, off, u_is_set, &tr_tree_bits);
-    if (tr_depth == 0 || cbf_is_set(tr_cu->cbf, depth - 1, 2)) cabac_bin(&c.S->tb, sc, off, v_is_set, &tr_tree_bits);
+    if (tr_depth == 0 || cbf_is_set(tr_cu->cbf, depth - 1, 1)) cabac_bin(&S->tb, sc, off, u_is_set, &tr_tree_bits);
+    if (tr_depth == 0 || cbf_is_set(tr_cu->cbf, depth - 1, 2)) cabac_bin(&S->tb, sc, off, v_is_set, &tr_tree_bits);
   }
   if (u_is_set) coeff_bits += coeff_bits_u;
   if (v_is_set) coeff_bits += coeff_bits_v;
   const double bits = tr_tree_bits + coeff_bits;
-  return (double)ssd * 1.5 + bits * c.cfg->lambda;
+  return (double)ssd * 1.5 + bits * S->cfg.lambda;
 }
 
 // the same with the coefficient bits taken from the level's (or staged) coefficients; S->ssd[leaf] holds the SSDs
-template <typename Pix> CTU_FN_NOINLINE double cu_rd_cost_chroma_leaf_of_level(const CtxT<Pix> &c, LcuLevel<Pix> *L, int xl, int yl, int depth, const CuRec *pred_cu, int leaf)
+template <typename Pix> CTU_FN_NOINLINE double cu_rd_cost_chroma_leaf_of_level(CtuST<Pix> *S, LcuLevel<Pix> *L, int xl, int yl, int depth, const CuRec *pred_cu, int leaf)
 {
   if (xl % 8 != 0 || yl % 8 != 0) return 0;
+  S = sm(S); L = sm(L); pred_cu = sm(pred_cu);
   const CuRec *tr_cu = cu_at(L, xl, yl);
   const int width = depth <= 3 ? (64 >> (depth + 1)) : (64 >> depth);
   const int scan = scan_order_intra(pred_cu->mode_chroma, depth);
   double bu = 0, bv = 0;
-  if (cbf_is_set(tr_cu->cbf, depth, 1)) bu = coeff_cost_of_unit(c, &c.S->sc, L, 1, xl, yl, depth, ilog2(width), 2, scan);
-  if (cbf_is_set(tr_cu->cbf, depth, 2)) bv = coeff_cost_of_unit(c, &c.S->sc, L, 2, xl, yl, depth, ilog2(width), 2, scan);
-  return cu_rd_cost_chroma_leaf(c, L, xl, yl, depth, pred_cu, c.S->ssd[leaf][1] + c.S->ssd[leaf][2], bu, bv);
+  if (cbf_is_set(tr_cu->cbf, depth, 1)) bu = coeff_cost_of_unit(S, &S->sc, L, 1, xl, yl, depth, ilog2(width), 2, scan);
+  if (cbf_is_set(tr_cu->cbf, depth, 2)) bv = coeff_cost_of_unit(S, &S->sc, L, 2, xl, yl, depth, ilog2(width), 2, scan);
+  return cu_rd_cost_chroma_leaf(S, L, xl, yl, depth, pred_cu, S->ssd[leaf][1] + S->ssd[leaf][2], bu, bv);
 }
 
-// cu_rd_cost_tr_split_accurate (ref: search.c:414-543), one node.  Leader only.  `leaf`: index into S->ssd.
-template <typename Pix> CTU_FN_NOINLINE double cost_accurate_node(const CtxT<Pix> &c, LcuLevel<Pix> *L, int xl, int yl, int depth, const CuRec *pred_cu, int leaf, bool *is_split)
+// cu_rd_cost_tr_split_accurate (ref: search.c:414-543), one node.  Leader only.  `leaf`: index into S->ssd.  A node
+// whose record is split further (tr_depth > depth) returns its tr_tree_bits only.
+template <typename Pix> CTU_FN_NOINLINE double cost_accurate_node(CtuST<Pix> *S, LcuLevel<Pix> *L, int xl, int yl, int depth, const CuRec *pred_cu, int leaf)
 {
-  const CtuST<Pix> *S = c.S;
-  CabacState *sc = &c.S->sc;
+  S = sm(S); L = sm(L); pred_cu = sm(pred_cu);
+  CabacState *sc = &S->sc;
   const int width = 64 >> depth;
   CuRec *tr_cu = cu_at(L, xl, yl);
   double coeff_bits = 0, tr_tree_bits = 0;
@@ -509,86 +525,84 @@ template <typename Pix> CTU_FN_NOINLINE double cost_accurate_node(const CtxT<Pix
   const bool intra_split_flag = pred_cu->part_size == SIZE_NxN && depth == 3;
   const int max_tr_depth = 0 + (intra_split_flag ? 1 : 0);
   if (width <= 32 && width > 4 && !intra_split_flag && imin((int)tr_cu->tr_depth, depth) - (int)tr_cu->depth < max_tr_depth)
-    cabac_bin(&c.S->tb, sc, CTX_TRANS_SUBDIV + (5 - (6 - depth)), tr_depth > 0, &tr_tree_bits);
+    cabac_bin(&S->tb, sc, CTX_TRANS_SUBDIV + (5 - (6 - depth)), tr_depth > 0, &tr_tree_bits);
   {
     const int off = CTX_CBF_CHROMA + (depth - (int)tr_cu->depth);
-    if ((int)tr_cu->depth == depth || cbf_is_set(tr_cu->cbf, depth - 1, 1)) cabac_bin(&c.S->tb, sc, off, cb_flag_u, &tr_tree_bits);
-    if ((int)tr_cu->depth == depth || cbf_is_set(tr_cu->cbf, depth - 1, 2)) cabac_bin(&c.S->tb, sc, off, cb_flag_v, &tr_tree_bits);
+    if ((int)tr_cu->depth == depth || cbf_is_set(tr_cu->cbf, depth - 1, 1)) cabac_bin(&S->tb, sc, off, cb_flag_u, &tr_tree_bits);
+    if ((int)tr_cu->depth == depth || cbf_is_set(tr_cu->cbf, depth - 1, 2)) cabac_bin(&S->tb, sc, off, cb_flag_v, &tr_tree_bits);
   }
-  *is_split = tr_depth > 0;
   if (tr_depth > 0) return tr_tree_bits;          // the caller sums the children and adds tr_tree_bits * lambda
   const int cb_flag_y = cbf_is_set(tr_cu->cbf, depth, 0);
   const int is_tr_split = depth - (int)tr_cu->depth;
-  cabac_bin(&c.S->tb, sc, CTX_CBF_LUMA + (is_tr_split ? 0 : 1), cb_flag_y, &tr_tree_bits);   // CU_INTRA
+  cabac_bin(&S->tb, sc, CTX_CBF_LUMA + (is_tr_split ? 0 : 1), cb_flag_y, &tr_tree_bits);   // CU_INTRA
   const unsigned luma_ssd = (unsigned)S->ssd[leaf][0];
   if (cb_flag_y) {
     const int scan = scan_order_intra(pred_cu->mode, depth);
-    coeff_bits += coeff_cost_of_unit(c, sc, L, 0, xl, yl, depth, ilog2(width), 0, scan);
+    coeff_bits += coeff_cost_of_unit(S, sc, L, 0, xl, yl, depth, ilog2(width), 0, scan);
   }
   unsigned chroma_ssd = 0;
   if (xl % 8 == 0 && yl % 8 == 0) {
     const int chroma_width = depth <= 3 ? (64 >> (depth + 1)) : (64 >> depth);
     chroma_ssd = (unsigned)S->ssd[leaf][1] + (unsigned)S->ssd[leaf][2];
     const int scan = scan_order_intra(pred_cu->mode_chroma, depth);
-    if (cb_flag_u) coeff_bits += coeff_cost_of_unit(c, sc, L, 1, xl, yl, depth, ilog2(chroma_width), 2, scan);
-    if (cb_flag_v) coeff_bits += coeff_cost_of_unit(c, sc, L, 2, xl, yl, depth, ilog2(chroma_width), 2, scan);
+    if (cb_flag_u) coeff_bits += coeff_cost_of_unit(S, sc, L, 1, xl, yl, depth, ilog2(chroma_width), 2, scan);
+    if (cb_flag_v) coeff_bits += coeff_cost_of_unit(S, sc, L, 2, xl, yl, depth, ilog2(chroma_width), 2, scan);
   }
   const double bits = tr_tree_bits + coeff_bits;
-  return luma_ssd * 0.8 + chroma_ssd * 1.5 + bits * c.cfg->lambda;
+  return luma_ssd * 0.8 + chroma_ssd * 1.5 + bits * S->cfg.lambda;
 }
-template <typename Pix> CTU_FN_NOINLINE double cost_tr_split_accurate(const CtxT<Pix> &c, LcuLevel<Pix> *L, int xl, int yl, int depth, const CuRec *pred_cu)
+template <typename Pix> CTU_FN_NOINLINE double cost_tr_split_accurate(CtuST<Pix> *S, LcuLevel<Pix> *L, int xl, int yl, int depth, const CuRec *pred_cu)
 {
-  bool split = false;
-  const double v = cost_accurate_node(c, L, xl, yl, depth, pred_cu, 0, &split);
+  S = sm(S); L = sm(L);
+  const bool split = (int)cu_at(L, xl, yl)->tr_depth > depth;       // (the cost walks do not change the records)
+  const double v = cost_accurate_node(S, L, xl, yl, depth, pred_cu, 0);
   if (!split) return v;
   const int offset = 64 >> (depth + 1);
   double sum = 0;
-  for (int k = 0; k < 4; ++k) {
-    bool s2 = false;
-    sum += cost_accurate_node(c, L, xl + (k & 1) * offset, yl + (k >> 1) * offset, depth + 1, pred_cu, k, &s2);
-  }
-  return sum + v * c.cfg->lambda;
+  for (int k = 0; k < 4; ++k) sum += cost_accurate_node(S, L, xl + (k & 1) * offset, yl + (k >> 1) * offset, depth + 1, pred_cu, k);
+  return sum + v * S->cfg.lambda;
 }
 
 // calc_mode_bits (ref: search.c:557-582).  Leader only.
-template <typename Pix> CTU_FN double calc_mode_bits(const CtxT<Pix> &c, LcuLevel<Pix> *L, const CuRec *cur_cu, int x, int y)
+template <typename Pix> CTU_FN double calc_mode_bits(CtuST<Pix> *S, LcuLevel<Pix> *L, const CuRec *cur_cu, int x, int y)
 {
   const int xl = x & 63, yl = y & 63;
   int8_t cand[3];
   const CuRec *left = x >= 4 ? cu_at(L, xl - 4, yl) : NULL;
   const CuRec *above = y >= 4 ? cu_at(L, xl, yl - 4) : NULL;
   intra_mpm(y, left, above, cand);
-  double mode_bits = luma_mode_bits(c, cur_cu->mode, cand);
-  if (x % 8 == 0 && y % 8 == 0) mode_bits += chroma_mode_bits(c, cur_cu->mode_chroma, cur_cu->mode);
+  double mode_bits = luma_mode_bits(S, cur_cu->mode, cand);
+  if (x % 8 == 0 && y % 8 == 0) mode_bits += chroma_mode_bits(S, cur_cu->mode_chroma, cur_cu->mode);
   return mode_bits;
 }
 
 // kvz_mock_encode_coding_unit for an intra CU in an I slice (ref: encode_coding_tree.c:977-1075, 464-652, 672-743).
 // Leader only.
-template <typename Pix> CTU_FN_NOINLINE double mock_encode_coding_unit(const CtxT<Pix> &c, LcuLevel<Pix> *L, int x, int y, int depth, const CuRec *cur_cu)
+template <typename Pix> CTU_FN_NOINLINE double mock_encode_coding_unit(CtuST<Pix> *S, LcuLevel<Pix> *L, int x, int y, int depth, const CuRec *cur_cu)
 {
+  S = sm(S); L = sm(L); cur_cu = sm(cur_cu);
   double bits = 0;
-  CabacState *sc = &c.S->sc;
+  CabacState *sc = &S->sc;
   const int xl = x & 63, yl = y & 63;
   const int cu_width = 64 >> depth;
   const CuRec *left_cu = x ? cu_at(L, xl - 1, yl) : NULL;
   const CuRec *above_cu = y ? cu_at(L, xl, yl - 1) : NULL;
-  const bool border = c.cfg->width < x + cu_width || c.cfg->height < y + cu_width;
+  const bool border = S->cfg.width < x + cu_width || S->cfg.height < y + cu_width;
   if (depth != 3 && !border) {
     int split_model = 0;
     if (left_cu && left_cu->depth > depth) ++split_model;
     if (above_cu && above_cu->depth > depth) ++split_model;
-    cabac_bin(&c.S->tb, sc, CTX_SPLIT + split_model, 0, &bits);
+    cabac_bin(&S->tb, sc, CTX_SPLIT + split_model, 0, &bits);
   }
   // kvz_encode_part_mode
   {
     double pb = 0;
-    if (depth == 3) cabac_bin(&c.S->tb, sc, CTX_PART_SIZE, cur_cu->part_size == SIZE_2Nx2N ? 1 : 0, &pb);
+    if (depth == 3) cabac_bin(&S->tb, sc, CTX_PART_SIZE, cur_cu->part_size == SIZE_2Nx2N ? 1 : 0, &pb);
     bits += pb;
   }
   // encode_intra_coding_unit in counting mode
   const int num_pu = cur_cu->part_size == SIZE_NxN ? 4 : 1;
-  int flag[4], mpm_idx[4];
+  unsigned flag = 0, mpm_nz = 0;    // bit j: PU j's mode is an MPM, it is not the first MPM
   int mode0 = 0;
   for (int j = 0; j < num_pu; ++j) {
     const int pw = num_pu == 4 ? cu_width / 2 : cu_width;
@@ -601,19 +615,20 @@ template <typename Pix> CTU_FN_NOINLINE double mock_encode_coding_unit(const Ctx
     intra_mpm(pu_y, left_pu, above_pu, preds);
     const int mode = cur_pu->mode;
     if (j == 0) mode0 = mode;
-    mpm_idx[j] = -1;
-    for (int i = 0; i < 3; ++i) if (preds[i] == mode) { mpm_idx[j] = i; break; }
-    flag[j] = mpm_idx[j] != -1;
+    int mpm_idx = -1;
+    for (int i = 0; i < 3; ++i) if (preds[i] == mode) { mpm_idx = i; break; }
+    if (mpm_idx != -1) flag |= 1u << j;
+    if (mpm_idx > 0) mpm_nz |= 1u << j;
   }
-  for (int j = 0; j < num_pu; ++j) cabac_bin(&c.S->tb, sc, CTX_INTRA_MODE, flag[j], &bits);
+  for (int j = 0; j < num_pu; ++j) cabac_bin(&S->tb, sc, CTX_INTRA_MODE, (flag >> j) & 1, &bits);
   for (int j = 0; j < num_pu; ++j) {
-    if (flag[j]) { bits += 1; if (mpm_idx[j] != 0) bits += 1; }
+    if ((flag >> j) & 1) { bits += 1; if ((mpm_nz >> j) & 1) bits += 1; }
     else bits += 5;
   }
   {
     const int mc = cur_cu->mode_chroma;
-    if (mc == mode0) cabac_bin(&c.S->tb, sc, CTX_CHROMA_PRED, 0, &bits);
-    else { cabac_bin(&c.S->tb, sc, CTX_CHROMA_PRED, 1, &bits); bits += 2; }
+    if (mc == mode0) cabac_bin(&S->tb, sc, CTX_CHROMA_PRED, 0, &bits);
+    else { cabac_bin(&S->tb, sc, CTX_CHROMA_PRED, 1, &bits); bits += 2; }
   }
   return bits;
 }
@@ -633,10 +648,11 @@ CTU_FN void sort_modes(int8_t *modes, double *costs, int length)
 
 // The per-mode quantities of search_intra_rough (get_cost / get_cost_dual, search_intra.c:89-160, and the mode bits
 // added at :524) for all 35 modes, one mode per thread.
-template <typename Pix> CTU_FN_NOINLINE void rough_mode_costs(const CtxT<Pix> &c, int log2w, const int8_t *mpm)
+template <typename Pix> CTU_FN_NOINLINE void rough_mode_costs(CtuST<Pix> *S, int log2w)
 {
-  CtuST<Pix> *S = c.S;
-  const CtuConfig *cfg = c.cfg;
+  S = sm(S);
+  const int8_t *mpm = S->mpm;
+  const CtuConfig *cfg = &S->cfg;
   const bool ts = log2w == 2 && cfg->trskip_enable;
   #pragma unroll 1
   for (int mode = CTU_TID; mode < 35; mode += CTU_NT) {
@@ -664,10 +680,11 @@ template <typename Pix> CTU_FN_NOINLINE void rough_mode_costs(const CtxT<Pix> &c
 }
 
 // search_intra_rough (ref: search_intra.c:391-530) replayed on the per-mode tables.  Leader only.
-template <typename Pix> CTU_FN_NOINLINE int rough_search_replay(const CtxT<Pix> &c, int log2w, const int8_t *mpm)
+template <typename Pix> CTU_FN_NOINLINE int rough_search_replay(CtuST<Pix> *S, int log2w)
 {
-  CtuST<Pix> *S = c.S;
-  const CtuConfig *cfg = c.cfg;
+  S = sm(S);
+  const int8_t *mpm = S->mpm;
+  const CtuConfig *cfg = &S->cfg;
   int8_t *modes = S->modes;
   double *costs = S->costs;
   int n = 0;
@@ -675,7 +692,7 @@ template <typename Pix> CTU_FN_NOINLINE int rough_search_replay(const CtxT<Pix> 
   int32_t min_cost = CTU_MAX_INT, max_cost = -CTU_MAX_INT - 1;
   int offset;
   if (cfg->full_intra_search) offset = 1;
-  else { const int offs[4] = { 2, 4, 8, 8 }; offset = offs[log2w - 2]; }
+  else offset = log2w == 2 ? 2 : (log2w == 3 ? 4 : 8);
   int best_mode = 2;
   double best_of_list = CTU_MAX_DOUBLE;
   for (int mode = 2; mode <= 34; mode += offset) {      // (mode, mode + offset) pairs of the reference's loop, in its order
@@ -695,6 +712,7 @@ template <typename Pix> CTU_FN_NOINLINE int rough_search_replay(const CtxT<Pix> 
       offset >>= 1;
       const int center = best_mode;
       const int test[2] = { center - offset, center + offset };
+      #pragma unroll
       for (int i = 0; i < 2; ++i) {
         if (test[i] >= 2 && test[i] <= 34) {
           costs[n] = S->rc0[test[i]];
@@ -707,6 +725,7 @@ template <typename Pix> CTU_FN_NOINLINE int rough_search_replay(const CtxT<Pix> 
     }
   }
   const int add_modes[5] = { mpm[0], mpm[1], mpm[2], 0, 1 };
+  #pragma unroll
   for (int p = 0; p < 5; ++p) {
     if (!((present >> add_modes[p]) & 1)) { costs[n] = S->rc1[add_modes[p]]; modes[n] = (int8_t)add_modes[p]; present |= 1ull << add_modes[p]; ++n; }
   }
@@ -726,10 +745,10 @@ template <typename Pix> CTU_FN_NOINLINE void keep_unit(Team tm, TuS<Pix> tu, Pix
 
 // kvz_search_cu_intra (ref: search_intra.c:806-900): best luma mode of the CU at (x, y, depth) on level L.
 // Result in S->best_mode / S->best_cost.
-template <typename Pix> CTU_FN_NOINLINE void search_cu_intra(const CtxT<Pix> &c, LcuLevel<Pix> *L, int x, int y, int depth)
+template <typename Pix> CTU_FN_NOINLINE void search_cu_intra(CtuST<Pix> *S, LcuLevel<Pix> *L, int x, int y, int depth)
 {
-  CtuST<Pix> *S = c.S;
-  const CtuConfig *cfg = c.cfg;
+  S = sm(S); L = sm(L);
+  const CtuConfig *cfg = &S->cfg;
   const int xl = x & 63, yl = y & 63;
   const int log2w = 6 - depth;
   CTU_LEADER {
@@ -741,16 +760,16 @@ template <typename Pix> CTU_FN_NOINLINE void search_cu_intra(const CtxT<Pix> &c,
   PROF_T0(PR_REFS);
   {
     // luma for the rough search; the chroma references the CU's reconstruction (and RDO candidates) will need as well
-    build_refs_multi(&c.S->tb, cfg->width, cfg->height, c.W, L, pack_log2w(log2w, tu_log2(depth, 1), tu_log2(depth, 2)), ((x & 4) || (y & 4)) ? 1 : 7, x, y, S->refs);
+    build_refs_multi(&S->tb, cfg->width, cfg->height, S->W, L, pack_log2w(log2w, tu_log2(depth, 1), tu_log2(depth, 2)), ((x & 4) || (y & 4)) ? 1 : 7, x, y, S->refs);
   }
   PROF_ADD(S, PR_REFS);
   // rough search: SATD (and SAD for 4x4 transform-skip candidates) of every mode, then the reference's selection
   PROF_T0(PR_SATD);
-  rough_costs_all_modes(&S->refs[0], (RoughExt<Pix> *)S->arena, log2w, 0, &c.W->src_y[yl * 64 + xl], 64, S->satd, S->sad, log2w == 2 && cfg->trskip_enable);
+  rough_costs_all_modes(&S->refs[0], (RoughExt<Pix> *)S->arena, log2w, 0, &S->W->src_y[yl * 64 + xl], 64, S->satd, S->sad, log2w == 2 && cfg->trskip_enable);
   PROF_ADD(S, PR_SATD);
   PROF_T0(PR_REPLAY);
-  rough_mode_costs(c, log2w, S->mpm);
-  CTU_LEADER S->n_modes = rough_search_replay(c, log2w, S->mpm);
+  rough_mode_costs(S, log2w);
+  CTU_LEADER S->n_modes = rough_search_replay(S, log2w);
   CTU_SYNC();
   PROF_ADD(S, PR_REPLAY);
   PROF_T0(PR_RDO_LOOP);
@@ -786,7 +805,7 @@ template <typename Pix> CTU_FN_NOINLINE void search_cu_intra(const CtxT<Pix> &c,
     // tasks: the luma units of all candidates (k: the transform-skip alternative), then (U, V) of each candidate, so
     // that the two halves of a warp get two luma units or the two chroma units of one candidate
     const int ntl = ncand * nluma;
-    for_tu_tasks(c, ntl + ncand * (np - 1), [&](int t) { return t < ntl ? tu_class(log2w, 0) : tu_class(tu_log2(depth, 1), 1); },
+    for_tu_tasks(S, ntl + ncand * (np - 1), [&](int t) { return t < ntl ? tu_class(log2w, 0) : tu_class(tu_log2(depth, 1), 1); },
                  [&](const Team &tm, unsigned char *slot, int t) {
       const int cand = t < ntl ? t / nluma : (t - ntl) >> 1;
       const int k = t < ntl ? t - cand * nluma : 0;
@@ -794,18 +813,18 @@ template <typename Pix> CTU_FN_NOINLINE void search_cu_intra(const CtxT<Pix> &c,
       const int mode = S->modes[cand];
       const int log2n = tu_log2(depth, col), n = 1 << log2n;
       const TuS<Pix> tu = tu_at<Pix>(slot, n * n);
-      const Plane<Pix> P = plane_of(c.W, L, col);
+      const Plane<Pix> P = plane_of(S->W, L, col);
       const int sh = col ? 1 : 0;
       const int off = (xl >> sh) + (yl >> sh) * P.lw;
       TuJob<Pix> j = { &S->refs[col], P.src + off, P.lw, col, log2n, mode, scan_order_intra(mode, depth), rdoq_tr_depth };
       int ts = 0;
-      if (col == 0 && ts_split) tu_core(tm, &c.S->tb, &S->tb, cfg, S->cabac0.ctx, tu, j, k == 1);
-      else ts = tu_eval(tm, &c.S->tb, &S->tb, cfg, S->cabac0.ctx, &S->sc, tu, j);
+      if (col == 0 && ts_split) tu_core(tm, &S->tb, &S->tb, cfg, S->cabac0.ctx, tu, j, k == 1);
+      else ts = tu_eval(tm, &S->tb, &S->tb, cfg, S->cabac0.ctx, &S->sc, tu, j);
       // keep the unit for write_back_candidate (not the chroma of depth 4, which is quantised again: see there)
       if (col == 0 || depth < 4) {
         const int unit = col == 0 ? cand * nluma + k : cand;
-        Pix *kr = (col == 0 ? c.W->cand.rec_y : c.W->cand.rec_c[col - 1]) + unit * n * n;
-        int16_t *kq = (col == 0 ? c.W->cand.q_y : c.W->cand.q_c[col - 1]) + unit * n * n;
+        Pix *kr = (col == 0 ? S->W->cand.rec_y : S->W->cand.rec_c[col - 1]) + unit * n * n;
+        int16_t *kq = (col == 0 ? S->W->cand.q_y : S->W->cand.q_c[col - 1]) + unit * n * n;
         keep_unit(tm, tu, kr, kq);
       }
       if (tm.tid == 0) {
@@ -815,7 +834,7 @@ template <typename Pix> CTU_FN_NOINLINE void search_cu_intra(const CtxT<Pix> &c,
         r->cg_mask = (uint64_t)fx->cg_mask[0] | ((uint64_t)fx->cg_mask[1] << 32);
         // coefficient bits of kvz_cu_rd_cost_luma / _chroma: the search models are not adapted here (update == 0)
         PROF_T0(PR_COEFFCOST);
-        r->bits = fx->has ? coeff_cost_serial(&c.S->tb, &S->tb, cfg, &S->sc, tu.q(), log2n, col ? 2 : 0, j.scan_idx, 0, r->cg_mask) : 0.0;
+        r->bits = fx->has ? coeff_cost_serial(&S->tb, &S->tb, cfg, &S->sc, tu.q(), log2n, col ? 2 : 0, j.scan_idx, 0, r->cg_mask) : 0.0;
         PROF_ADD(S, PR_COEFFCOST);
       }
       tsync(tm);
@@ -836,7 +855,7 @@ template <typename Pix> CTU_FN_NOINLINE void search_cu_intra(const CtxT<Pix> &c,
           S->res[r][0].tr_skip = pick;
         }
         const int mode = S->modes[r];
-        const double rdo_bitcost = luma_mode_bits(c, mode, S->mpm);
+        const double rdo_bitcost = luma_mode_bits(S, mode, S->mpm);
         S->costs[r] = rdo_bitcost * cfg->lambda;
         CuRec *p = &S->pred_cu;
         p->depth = (uint8_t)depth; p->type = CU_INTRA; p->part_size = depth == 4 ? SIZE_NxN : SIZE_2Nx2N;
@@ -845,8 +864,8 @@ template <typename Pix> CTU_FN_NOINLINE void search_cu_intra(const CtxT<Pix> &c,
         // the level's record carries the candidate's cbf bits (cbf_copy in kvz_intra_recon_cu's leaf)
         for (int col = 0; col < np; ++col) cbf_copy(&tr_cu->cbf, p->cbf, col);
         double nosplit = 0.0;
-        nosplit += cu_rd_cost_luma_leaf(c, L, xl, yl, depth, p, S->res[r][0].ssd, S->res[r][0].bits);
-        if (reconstruct_chroma) nosplit += cu_rd_cost_chroma_leaf(c, L, xl, yl, depth, p, S->res[r][1].ssd + S->res[r][2].ssd, S->res[r][1].bits, S->res[r][2].bits);
+        nosplit += cu_rd_cost_luma_leaf(S, L, xl, yl, depth, S->res[r][0].ssd, S->res[r][0].bits);
+        if (reconstruct_chroma) nosplit += cu_rd_cost_chroma_leaf(S, L, xl, yl, depth, p, S->res[r][1].ssd + S->res[r][2].ssd, S->res[r][1].bits, S->res[r][2].bits);
         S->costs[r] += nosplit;
         if (cfg->intra_rdo_et && !cbf_is_set_any(p->cbf, depth)) { S->n_modes = r + 1; break; }
       }
@@ -872,27 +891,28 @@ template <typename Pix> CTU_FN_NOINLINE void search_cu_intra(const CtxT<Pix> &c,
 }
 
 // kvz_search_cu_intra_chroma (ref: search_intra.c:748-803) for rdo 2..3 (num_modes = 2).  Returns the mode (uniform).
-template <typename Pix> CTU_FN_NOINLINE int search_cu_intra_chroma(const CtxT<Pix> &c, LcuLevel<Pix> *L, int x, int y, int depth)
+template <typename Pix> CTU_FN_NOINLINE int search_cu_intra_chroma(CtuST<Pix> *S, LcuLevel<Pix> *L, int x, int y, int depth)
 {
-  CtuST<Pix> *S = c.S;
+  S = sm(S); L = sm(L);
   const int xl = x & 63, yl = y & 63;
   const int intra_mode = cu_at(L, xl, yl)->mode;
   const int log2wc = imax(6 - depth - 1, 2);
   const int wc = 1 << log2wc;
   CTU_LEADER {
     const int8_t init[5] = { 0, 26, 10, 1, 34 };
+    #pragma unroll
     for (int i = 0; i < 5; ++i) S->cmodes[i] = init[i];
     if (intra_mode != 0 && intra_mode != 26 && intra_mode != 10 && intra_mode != 1) S->cmodes[4] = (int8_t)intra_mode;
   }
   CTU_SYNC();
-  build_refs(&c.S->tb, c.cfg, c.W, L, log2wc, 1, x, y, &S->refs[1]);
-  build_refs(&c.S->tb, c.cfg, c.W, L, log2wc, 2, x, y, &S->refs[2]);
+  build_refs(&S->tb, &S->cfg, S->W, L, log2wc, 1, x, y, &S->refs[1]);
+  build_refs(&S->tb, &S->cfg, S->W, L, log2wc, 2, x, y, &S->refs[2]);
   // search_intra_chroma_rough: SATD of the five candidates on U and V (the luma mode is skipped: cost 0)
   const int ci = (yl >> 1) * 32 + (xl >> 1);
-  rough_costs_all_modes(&S->refs[1], (RoughExt<Pix> *)S->arena, log2wc, 1, &c.W->src_u[ci], 32, S->satd, S->sad, false);
+  rough_costs_all_modes(&S->refs[1], (RoughExt<Pix> *)S->arena, log2wc, 1, &S->W->src_u[ci], 32, S->satd, S->sad, false);
   CTU_LEADER { for (int i = 0; i < 5; ++i) S->ccosts[i] = 0; for (int i = 0; i < 5; ++i) if (S->cmodes[i] != intra_mode) S->ccosts[i] += (double)(unsigned)S->satd[S->cmodes[i]]; }
   CTU_SYNC();
-  rough_costs_all_modes(&S->refs[2], (RoughExt<Pix> *)S->arena, log2wc, 2, &c.W->src_v[ci], 32, S->satd, S->sad, false);
+  rough_costs_all_modes(&S->refs[2], (RoughExt<Pix> *)S->arena, log2wc, 2, &S->W->src_v[ci], 32, S->satd, S->sad, false);
   CTU_LEADER {
     for (int i = 0; i < 5; ++i) if (S->cmodes[i] != intra_mode) S->ccosts[i] += (double)(unsigned)S->satd[S->cmodes[i]];
     sort_modes(S->cmodes, S->ccosts, 5);
@@ -904,7 +924,7 @@ template <typename Pix> CTU_FN_NOINLINE int search_cu_intra_chroma(const CtxT<Pi
   int best_mode = 0;
   for (int i = 0; i < 2; ++i) {
     const int mode = S->cmodes[i];
-    intra_recon_cu(c, L, x, y, depth, -1, mode, NULL, (depth == 0 ? 0 : 6) | ((intra_mode + 1) << 8));
+    intra_recon_cu(S, L, x, y, depth, -1, mode, NULL, (depth == 0 ? 0 : 6) | ((intra_mode + 1) << 8));
     CTU_LEADER {
       CuRec *tr_cu = cu_at(L, xl, yl);
       double cost;
@@ -913,17 +933,17 @@ template <typename Pix> CTU_FN_NOINLINE int search_cu_intra_chroma(const CtxT<Pi
         CabacState *sc = &S->sc;
         double tr_tree_bits = 0;
         if (!sc->update || tr_cu->tr_depth != tr_cu->depth) {
-          cabac_bin(&c.S->tb, sc, CTX_CBF_CHROMA, cbf_is_set(tr_cu->cbf, 0, 1), &tr_tree_bits);
-          cabac_bin(&c.S->tb, sc, CTX_CBF_CHROMA, cbf_is_set(tr_cu->cbf, 0, 2), &tr_tree_bits);
+          cabac_bin(&S->tb, sc, CTX_CBF_CHROMA, cbf_is_set(tr_cu->cbf, 0, 1), &tr_tree_bits);
+          cabac_bin(&S->tb, sc, CTX_CBF_CHROMA, cbf_is_set(tr_cu->cbf, 0, 2), &tr_tree_bits);
         }
         double sum = 0;
-        for (int k = 0; k < 4; ++k) sum += cu_rd_cost_chroma_leaf_of_level(c, L, xl + (k & 1) * 32, yl + (k >> 1) * 32, 1, tr_cu, k);
-        cost = sum + tr_tree_bits * c.cfg->lambda;
+        for (int k = 0; k < 4; ++k) sum += cu_rd_cost_chroma_leaf_of_level(S, L, xl + (k & 1) * 32, yl + (k >> 1) * 32, 1, tr_cu, k);
+        cost = sum + tr_tree_bits * S->cfg.lambda;
       } else {
-        cost = cu_rd_cost_chroma_leaf_of_level(c, L, xl, yl, depth, tr_cu, 0);
+        cost = cu_rd_cost_chroma_leaf_of_level(S, L, xl, yl, depth, tr_cu, 0);
       }
-      const double mode_bits = chroma_mode_bits(c, mode, intra_mode);
-      cost += mode_bits * c.cfg->lambda;
+      const double mode_bits = chroma_mode_bits(S, mode, intra_mode);
+      cost += mode_bits * S->cfg.lambda;
       S->ccosts[5 + i] = cost;
     }
     CTU_SYNC();
@@ -941,18 +961,18 @@ template <typename Pix> CTU_FN int split_model_of(LcuLevel<Pix> *L, int x, int y
   return (condA ? 1 : 0) + (condL ? 1 : 0);
 }
 
-// search_cu for the whole CTU at (cx, cy) (luma picture coordinates); returns with the decisions on level 0
-template <typename Pix> CTU_FN_NOINLINE void search_ctu(const CtxT<Pix> &c, int cx, int cy)
+// search_cu for the whole CTU at (cx, cy) (luma picture coordinates); returns with the decisions on level 0.  The
+// caller has loaded the tables into S->tb.
+template <typename Pix> CTU_FN_NOINLINE void search_ctu(CtuST<Pix> *S, int cx, int cy)
 {
-  CtuST<Pix> *S = c.S;
-  const CtuConfig *cfg = c.cfg;
-  sm_tables_load(&S->tb, c.T);
+  S = sm(S);
+  const CtuConfig *cfg = &S->cfg;
   CTU_LEADER { S->fr[0].x = cx; S->fr[0].y = cy; S->fr[0].stage = 0; S->stage_key[0] = S->stage_key[1] = S->stage_key[2] = -1; }
   CTU_SYNC();
   int d = 0;
   for (;;) {
     SearchFrame *F = &S->fr[d];
-    LcuLevel<Pix> *L = &c.S->lv[d];
+    LcuLevel<Pix> *L = &S->lv[d];
     // Every thread takes its copy of the frame's state, THEN the barrier: the leader changes that state below, and a
     // thread that read it late would take another branch than the others (all control flow here must be uniform).
     const int x = F->x, y = F->y;
@@ -990,7 +1010,7 @@ template <typename Pix> CTU_FN_NOINLINE void search_ctu(const CtxT<Pix> &c, int 
         const bool can_use_intra = (d >= cfg->pu_depth_intra_min && d <= cfg->pu_depth_intra_max) ||
                                    (x & ~(cwim - 1)) + cwim > cfg->width || (y & ~(cwim - 1)) + cwim > cfg->height;
         if (can_use_intra) {
-          search_cu_intra(c, L, x, y, d);
+          search_cu_intra(S, L, x, y, d);
           CTU_LEADER {
             if (S->best_cost < F->cost) {
               F->cost = S->best_cost;
@@ -1009,20 +1029,20 @@ template <typename Pix> CTU_FN_NOINLINE void search_ctu(const CtxT<Pix> &c, int 
           // the references search_cu_intra built are still this CU's
           const int refs_valid = aligned ? 7 : 1;
           if (aligned && cfg->rdo >= 2 && cfg->intra_chroma_search) {
-            intra_recon_cu(c, L, x, y, d, cur_cu->mode, -1, NULL, refs_valid);
+            intra_recon_cu(S, L, x, y, d, cur_cu->mode, -1, NULL, refs_valid);
             PROF_T0(PR_CHROMA);
-            const int mc = search_cu_intra_chroma(c, L, x, y, d);
+            const int mc = search_cu_intra_chroma(S, L, x, y, d);
             PROF_ADD(S, PR_CHROMA);
             CTU_LEADER cur_cu->mode_chroma = (int8_t)mc;
             CTU_SYNC();
             fill_cu_info(L, xl, yl, cu_width, cur_cu);
-            intra_recon_cu(c, L, x, y, d, -1, cur_cu->mode_chroma, NULL, 0);
+            intra_recon_cu(S, L, x, y, d, -1, cur_cu->mode_chroma, NULL, 0);
           } else if (cfg->rdo >= 2) {
             // the winner's reconstruction is the one its RDO candidate computed (a leaf: depth >= 1, tr_depth == depth)
-            write_back_candidate(c, L, x, y, d, cur_cu->mode, aligned);
+            write_back_candidate(S, L, x, y, d, cur_cu->mode, aligned);
           } else {
             // luma and chroma of the CU are independent: one pass (kvz_intra_recon_cu twice in the reference)
-            intra_recon_cu(c, L, x, y, d, cur_cu->mode, aligned ? cur_cu->mode_chroma : -1, NULL, refs_valid);
+            intra_recon_cu(S, L, x, y, d, cur_cu->mode, aligned ? cur_cu->mode_chroma : -1, NULL, refs_valid);
           }
         }
       }
@@ -1031,10 +1051,10 @@ template <typename Pix> CTU_FN_NOINLINE void search_ctu(const CtxT<Pix> &c, int 
         CTU_LEADER {
           double bits = 0;
           S->sc.update = 1;
-          if (cur_cu->part_size == SIZE_2Nx2N) bits += mock_encode_coding_unit(c, L, x, y, d, cur_cu);
-          else bits += calc_mode_bits(c, L, cur_cu, x, y);
+          if (cur_cu->part_size == SIZE_2Nx2N) bits += mock_encode_coding_unit(S, L, x, y, d, cur_cu);
+          else bits += calc_mode_bits(S, L, cur_cu, x, y);
           double cost = bits * cfg->lambda;
-          cost += cost_tr_split_accurate(c, L, xl, yl, d, cur_cu);
+          cost += cost_tr_split_accurate(S, L, xl, yl, d, cur_cu);
           F->cost = cost;
           S->sc.update = 0;
         }
@@ -1053,8 +1073,8 @@ template <typename Pix> CTU_FN_NOINLINE void search_ctu(const CtxT<Pix> &c, int 
           S->sc = F->pre;
           S->sc.update = 1;
           double split_bits = 0;
-          if (d < 3) cabac_bin(&c.S->tb, &S->sc, CTX_SPLIT + split_model_of(L, x, y, d), 1, &split_bits);
-          if (cur_cu->type == CU_INTRA && d == 3) cabac_bin(&c.S->tb, &S->sc, CTX_PART_SIZE, 0, &split_bits);
+          if (d < 3) cabac_bin(&S->tb, &S->sc, CTX_SPLIT + split_model_of(L, x, y, d), 1, &split_bits);
+          if (cur_cu->type == CU_INTRA && d == 3) cabac_bin(&S->tb, &S->sc, CTX_PART_SIZE, 0, &split_bits);
           S->sc.update = 0;
           F->split_cost += split_bits * cfg->lambda;
           if (cur_cu->type == CU_NOTSET || F->cbf || cfg->cu_split_termination == 1) F->do_children = 1;
@@ -1066,7 +1086,7 @@ template <typename Pix> CTU_FN_NOINLINE void search_ctu(const CtxT<Pix> &c, int 
       CTU_SYNC();
       if (!can_split) {
         // no split possible at this depth: the CU is final, return to the parent at once
-        if (d < 4) work_tree_copy_down(c, xl, yl, d);
+        if (d < 4) work_tree_copy_down(S, xl, yl, d);
         if (d == 0) break;
         --d;
         CTU_LEADER S->fr[d].split_cost += S->ret_cost;
@@ -1093,19 +1113,19 @@ template <typename Pix> CTU_FN_NOINLINE void search_ctu(const CtxT<Pix> &c, int 
       const bool inside = x + cu_width <= cfg->width && y + cu_width <= cfg->height;
       bool combine = false;
       if (cur_cu->type == CU_NOTSET && d < 4 && inside && cfg->combine_intra_cus) {
-        const CuRec *cu_d1 = cu_at(&c.S->lv[d + 1], xl, yl);
+        const CuRec *cu_d1 = cu_at(&S->lv[d + 1], xl, yl);
         combine = cu_d1->type == CU_INTRA && cu_d1->depth == d + 1;
       }
       CTU_SYNC();       // (the decision is taken by everybody before the leader rewrites the record)
       if (combine) {
-        CuRec *cu_d1 = cu_at(&c.S->lv[d + 1], xl, yl);
+        CuRec *cu_d1 = cu_at(&S->lv[d + 1], xl, yl);
         {
           CTU_LEADER {
             S->tmp = S->sc;
             S->sc = F->pre;
             F->cost = 0;
             double bits = 0;
-            if (d < 3) cabac_bin(&c.S->tb, &S->sc, CTX_SPLIT + split_model_of(L, x, y, d), 0, &bits);
+            if (d < 3) cabac_bin(&S->tb, &S->sc, CTX_SPLIT + split_model_of(L, x, y, d), 0, &bits);
             S->best_cost = bits;
             cur_cu->mode = cu_d1->mode; cur_cu->mode_chroma = cu_d1->mode_chroma;
             cur_cu->type = CU_INTRA;
@@ -1114,12 +1134,12 @@ template <typename Pix> CTU_FN_NOINLINE void search_ctu(const CtxT<Pix> &c, int 
           CTU_SYNC();
           fill_trdepth(L, xl, yl, d, cur_cu->tr_depth);
           fill_cu_info(L, xl, yl, cu_width, cur_cu);
-          intra_recon_cu(c, L, x, y, d, cur_cu->mode, cur_cu->mode_chroma, NULL, 0);
+          intra_recon_cu(S, L, x, y, d, cur_cu->mode, cur_cu->mode_chroma, NULL, 0);
           CTU_LEADER {
-            const double mode_bits = calc_mode_bits(c, L, cur_cu, x, y) + S->best_cost;
+            const double mode_bits = calc_mode_bits(S, L, cur_cu, x, y) + S->best_cost;
             double cost = F->cost;
             cost += mode_bits * cfg->lambda;
-            cost += cost_tr_split_accurate(c, L, xl, yl, d, cur_cu);
+            cost += cost_tr_split_accurate(S, L, xl, yl, d, cur_cu);
             F->cost = cost;
             F->post = S->sc;
             S->sc = S->tmp;
@@ -1132,11 +1152,11 @@ template <typename Pix> CTU_FN_NOINLINE void search_ctu(const CtxT<Pix> &c, int 
       if (split_wins) {
         CTU_LEADER F->cost = F->split_cost;
         CTU_SYNC();
-        work_tree_copy_up(c, xl, yl, d);
+        work_tree_copy_up(S, xl, yl, d);
       } else if (d > 0) {
         CTU_LEADER S->sc = F->post;
         CTU_SYNC();
-        work_tree_copy_down(c, xl, yl, d);
+        work_tree_copy_down(S, xl, yl, d);
       }
     }
     // return to the parent

@@ -38,7 +38,7 @@ constexpr int kThreads = 128;
 static_assert(sizeof(CtuST<uint8_t>) + 1024 + 64 <= 228 * 1024 / 3, "CtuST<uint8_t> no longer fits three CTAs per SM");
 static_assert(sizeof(CtuST<uint16_t>) + 1024 + 64 <= 228 * 1024 / 3, "CtuST<uint16_t> no longer fits three CTAs per SM");
 #if !defined(KVZ_CTU_PROF)
-static_assert(sizeof(CtuST<uint8_t>) == 74960, "the 8-bit shared-memory layout changed");
+static_assert(sizeof(CtuST<uint8_t>) == 75072, "the 8-bit shared-memory layout changed");
 #endif
 
 template <typename Pix> struct KernelArgs {
