@@ -36,10 +36,18 @@ $(LIB): $(OBJS)
 # compared with; never linked into the product library
 PROBE     := tests/cuda/libkvzctu_probe.so
 PROBE_HOST := tests/hostsim/libkvzctu_probe_host.so
-probe: $(PROBE) $(PROBE_HOST)
+# ... and the back half of its CTU job (deblocking, SAO search and application, model tracking) on injected decisions
+# (tests/test_ctu_frame_stage.py), the same two builds
+FPROBE    := tests/cuda/libkvzctu_frame_probe.so
+FPROBE_HOST := tests/hostsim/libkvzctu_frame_probe_host.so
+probe: $(PROBE) $(PROBE_HOST) $(FPROBE) $(FPROBE_HOST)
 $(PROBE): tests/cuda/ctu_tu_probe.cu $(wildcard $(SRCDIR)/*.h) $(wildcard $(SRCDIR)/ctu/*.h)
 	$(NVCC) $(ARCH) -O3 -std=c++17 -fmad=false -Xcompiler -fPIC,-Wall -shared -o $@ $< -lcudart
 $(PROBE_HOST): tests/cuda/ctu_tu_probe.cu $(wildcard $(SRCDIR)/*.h) $(wildcard $(SRCDIR)/ctu/*.h)
+	g++ -O2 -g -std=c++17 -fPIC -shared -ffp-contract=off -Wall -Wno-unused-function -Wno-unknown-pragmas -x c++ -o $@ $<
+$(FPROBE): tests/cuda/ctu_frame_probe.cu $(wildcard $(SRCDIR)/*.h) $(wildcard $(SRCDIR)/ctu/*.h)
+	$(NVCC) $(ARCH) -O3 -std=c++17 -fmad=false -Xcompiler -fPIC,-Wall -shared -o $@ $< -lcudart
+$(FPROBE_HOST): tests/cuda/ctu_frame_probe.cu $(wildcard $(SRCDIR)/*.h) $(wildcard $(SRCDIR)/ctu/*.h)
 	g++ -O2 -g -std=c++17 -fPIC -shared -ffp-contract=off -Wall -Wno-unused-function -Wno-unknown-pragmas -x c++ -o $@ $<
 
 oracle:
@@ -48,4 +56,4 @@ ref:
 	$(MAKE) -s -C oracle ref
 
 clean:
-	rm -rf build $(LIB) $(PROBE) $(PROBE_HOST)
+	rm -rf build $(LIB) $(PROBE) $(PROBE_HOST) $(FPROBE) $(FPROBE_HOST)
