@@ -7,7 +7,7 @@
 //     macro lists, expanded into host arrays (ctu_tables_init) and device arrays (the strategy kernels);
 //   * scalar rules: kvz_get_scaled_qp, the scan order of a block of up to 8x8, the last-position group index;
 //   * context-model offsets into the kvz_cuda_cabac_ctx image;
-//   * RDOQ: level rate, significance context, sign hiding;
+//   * RDOQ: level rate, significance context, sign hiding; kvz_quant's sign hiding;
 //   * the CABAC bit count of a transform unit (kvz_get_coeff_cost's CABAC branch).
 #pragma once
 #include <stdint.h>
@@ -294,6 +294,40 @@ COEFF_FN void rdoq_sign_hiding(const int32_t *s_inc, const int32_t *s_dec, const
     if (coef[best_pos] >= 0) q[best_pos] = (int16_t)(q[best_pos] + best_change);
     else q[best_pos] = (int16_t)(q[best_pos] - best_change);
   }
+}
+
+// kvz_quant's sign-bit hiding of coefficient group g (quant-generic.c:84-176).  pos[k]: raster position of scan position
+// 16 * g + k, wherever the caller takes the scan from; delta_u: the rounding remainders of kvz_quant by raster
+// position; cg_nz[h]: whether group h had a non-zero level before any hiding.  Groups only interact through "is this
+// the last non-zero group of the scan", so one thread per group is race free.
+template <class PosT, class NzT>
+COEFF_FN void quant_sign_hiding(const PosT *pos, const int16_t *coef, int16_t *q, const int32_t *delta_u, const NzT *cg_nz, int num_cg, int g)
+{
+  bool last_cg = true;
+  for (int h = g + 1; h < num_cg; ++h) if (cg_nz[h]) { last_cg = false; break; }
+  int first_nz = 16, last_nz = -1, abssum = 0;
+  for (int k = 15; k >= 0; --k) if (q[pos[k]]) { last_nz = k; break; }
+  for (int k = 0; k < 16; ++k) if (q[pos[k]]) { first_nz = k; break; }
+  for (int k = first_nz; k <= last_nz; ++k) abssum += q[pos[k]];
+  if (last_nz - first_nz < 4) return;
+  const int signbit = q[pos[first_nz]] > 0 ? 0 : 1;
+  if (signbit == (abssum & 1)) return;
+  int min_cost = 0x7fffffff, cur_cost = 0x7fffffff, min_pos = -1;
+  int final_change = 0, cur_change = 0;
+  for (int k = (last_cg ? last_nz : 15); k >= 0; --k) {
+    const int b = pos[k];
+    if (q[b] != 0) {
+      if (delta_u[b] > 0) { cur_cost = -delta_u[b]; cur_change = 1; }
+      else if (k == first_nz && iabs((int)q[b]) == 1) { cur_cost = 0x7fffffff; }
+      else { cur_cost = delta_u[b]; cur_change = -1; }
+    } else if (k < first_nz && ((coef[b] >= 0) ? 0 : 1) != signbit) {
+      cur_cost = 0x7fffffff;
+    } else { cur_cost = -delta_u[b]; cur_change = 1; }
+    if (cur_cost < min_cost) { min_cost = cur_cost; final_change = cur_change; min_pos = b; }
+  }
+  if (q[min_pos] == 32767 || q[min_pos] == -32768) final_change = -1;
+  if (coef[min_pos] >= 0) q[min_pos] = (int16_t)(q[min_pos] + final_change);
+  else q[min_pos] = (int16_t)(q[min_pos] - final_change);
 }
 
 // ---------------------------------------------------------------------------------------------- coefficient bits

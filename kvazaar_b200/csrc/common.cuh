@@ -7,8 +7,11 @@
 #include <atomic>
 
 #include "../../include/kvz_cuda.h"
+#include "pixel_rules.h"
 
 namespace kvzc {
+
+using namespace kvzpix;       // sample traits and the sample-domain rules shared with the CTU search
 
 // ---------------------------------------------------------------- host side
 extern std::atomic<uint64_t> g_launches;
@@ -109,10 +112,6 @@ int coeff_cost_launch_grid(int signhide, const kvz_cuda_cabac_ctx *ctx_dev, cons
                            const int8_t *modes, int trskip_enable, double *bits_out, double *bits_out2, cudaStream_t st, int is_chroma = 0);
 
 // ---------------------------------------------------------------- device side
-template <class T> struct PixTraits;
-template <> struct PixTraits<uint8_t> { static constexpr int kBits = 8; };
-template <> struct PixTraits<uint16_t> { static constexpr int kBits = 10; };
-
 __device__ __forceinline__ int warp_sum(int v)
 {
 #pragma unroll
@@ -136,5 +135,18 @@ __device__ __forceinline__ int block_sum(int v)
 }
 
 __device__ __forceinline__ int clip3(int lo, int hi, int v) { return min(max(v, lo), hi); }
+
+// the five offsets of an SAO edge class (categories 0..4) in registers, looked up by selection: an array indexed at run
+// time would live in local memory
+struct EdgeOffsets {
+  int o[5];
+  __device__ __forceinline__ int operator[](int cat) const
+  {
+    int v = o[0];
+#pragma unroll
+    for (int k = 1; k < 5; ++k) v = cat == k ? o[k] : v;
+    return v;
+  }
+};
 
 }  // namespace kvzc

@@ -15,6 +15,7 @@
 #include <stddef.h>
 #include <string.h>
 #include "../coeff_rules.h"
+#include "../pixel_rules.h"
 
 #if defined(__CUDACC__)
 #define CTU_FN __device__ __forceinline__
@@ -98,18 +99,8 @@ enum { PR_LOAD, PR_SEARCH, PR_STORE, PR_DEBLOCK, PR_SAO, PR_TRACK, PR_REFS, PR_S
 namespace kvzctu {
 
 using namespace kvzcoeff;
-
-// ---------------------------------------------------------------------------------------------- sample type
-// The algorithm is compiled once per sample type: uint8_t for 8-bit, uint16_t for 10-bit pictures (kvz_pixel of the
-// reference's KVZ_BIT_DEPTH builds).  Everything that depends on the bit depth is derived from the type at compile time.
-template <typename Pix> struct PixDepth;
-template <> struct PixDepth<uint8_t> { static constexpr int bd = 8; };
-template <> struct PixDepth<uint16_t> { static constexpr int bd = 10; };
-template <typename Pix> struct PixTraits {
-  static constexpr int bd = PixDepth<Pix>::bd;
-  static constexpr int max = (1 << bd) - 1;                           // CLIP_TO_PIXEL (ref: global.h)
-  static constexpr int sao_max = (1 << ((bd < 10 ? bd : 10) - 5)) - 1;  // SAO_ABS_OFFSET_MAX (ref: global.h:230)
-};
+// The algorithm is compiled once per sample type (PixTraits): uint8_t for 8-bit, uint16_t for 10-bit pictures.
+using namespace kvzpix;
 
 // ---------------------------------------------------------------------------------------------- configuration
 // Mirrors the fields of kvz_config / encoder_control_t / encoder_state_t the intra CTU search reads
@@ -222,18 +213,8 @@ struct CtuTables {
 };
 
 // ---- host-side table construction (product host code and the test build share it)
-namespace tables_detail {
-inline int zidx16(int ux, int uy)
-{
-  int z = 0;
-  for (int b = 0; b < 4; ++b) z |= (((ux >> b) & 1) << (2 * b)) | (((uy >> b) & 1) << (2 * b + 1));
-  return z;
-}
-}  // namespace tables_detail
-
 inline void ctu_tables_init(CtuTables *t)
 {
-  using namespace tables_detail;
   memset(t, 0, sizeof(*t));
   for (int s = 0; s < 3; ++s)
     for (int l = 2; l <= 5; ++l) {
@@ -255,13 +236,8 @@ inline void ctu_tables_init(CtuTables *t)
     }
   for (int uy = 0; uy < 16; ++uy)
     for (int ux = 0; ux < 16; ++ux) {
-      const int z = zidx16(ux, uy);
-      int n = 0;
-      if (uy == 0) n = 16; else while (ux + n < 16 && zidx16(ux + n, uy - 1) < z) ++n;
-      t->ref_top[uy][ux] = (uint8_t)(4 * n);
-      n = 0;
-      if (ux == 0) n = 16 - uy; else while (uy + n < 16 && zidx16(ux - 1, uy + n) < z) ++n;
-      t->ref_left[uy][ux] = (uint8_t)(4 * n);
+      t->ref_top[uy][ux] = (uint8_t)ref_px_top(uy, ux);
+      t->ref_left[uy][ux] = (uint8_t)ref_px_left(uy, ux);
     }
   static const int8_t c32[33] = { 64, 90, 90, 90, 89, 88, 87, 85, 83, 82, 80, 78, 75, 73, 70, 67, 64,
                                   61, 57, 54, 50, 46, 43, 38, 36, 31, 25, 22, 18, 13, 9, 4, 0 };
@@ -289,10 +265,6 @@ inline void ctu_tables_init(CtuTables *t)
   memcpy(t->min_in_group, mig, 10);
 }
 
-// ---------------------------------------------------------------------------------------------- small helpers
-CTU_FN int imax(int a, int b) { return a > b ? a : b; }
-CTU_FN int iclip(int lo, int hi, int v) { return v < lo ? lo : (v > hi ? hi : v); }
-
 // kvz_get_scan_order (ref: src/encoderstate.c:1761-1775), CU_INTRA only
 CTU_FN int scan_order_intra(int mode, int depth)
 {
@@ -305,6 +277,6 @@ CTU_FN int scan_order_intra(int mode, int depth)
 
 // kvz_get_scaled_qp with the qp_offset of the bit depth, 6 * (bd - 8) (ref: quant-generic.c:57, 305; rdo.c:672); the
 // search's QP is never negative, so the offset can be added after the chroma mapping
-template <typename Pix> CTU_FN int scaled_qp_px(int type, int qp) { return scaled_qp(type, qp, 0) + 6 * (PixDepth<Pix>::bd - 8); }
+template <typename Pix> CTU_FN int scaled_qp_px(int type, int qp) { return scaled_qp(type, qp, 0) + 6 * (PixTraits<Pix>::bd - 8); }
 
 }  // namespace kvzctu

@@ -172,11 +172,9 @@ template <typename Pix> CTU_FN_NOINLINE void ctu_store(CtuST<Pix> *S, const Fram
 }
 
 // ------------------------------------------------------------------------------------------------ deblocking
-CTU_FN int dbk_beta(int i) { return i < 16 ? 0 : (i < 29 ? i - 10 : 2 * i - 38); }
 CTU_FN int dbk_tc(int i)
 {
-  const uint8_t t[54] = { 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 1, 1, 1, 1, 1, 1, 1, 1, 1, 2, 2, 2, 2, 3, 3, 3, 3, 4, 4,
-                          4, 5, 5, 6, 6, 7, 8, 9, 10, 11, 13, 14, 16, 18, 20, 22, 24 };
+  const uint8_t t[54] = { PIX_DBK_TC };
   return t[i];
 }
 template <typename Pix> CTU_FN const CuRec *fcu(const FrameDevT<Pix> *F, int x, int y) { return &F->cu[(y >> 2) * F->cu_stride + (x >> 2)]; }
@@ -192,52 +190,11 @@ template <typename Pix> CTU_FN bool dbk_edge_wanted(const FrameDevT<Pix> *F, int
   return pos == cu_pos;       // (the inner PU boundary of NxN lies off the 8x8 grid)
 }
 
-// luma part of 4 lines: px -> q0 of line 0; xs across the edge, ys along it (ref: filter.c:95-170, 474-520)
-template <typename Pix> CTU_FN_NOINLINE void dbk_luma_part(Pix *px, int xs, int ys, int beta, int tc)
-{
-  int b[4][8];
-  for (int l = 0; l < 4; ++l) for (int i = 0; i < 8; ++i) b[l][i] = CTU_LD_FRAME(&px[l * ys + (i - 4) * xs]);
-  const int dp0 = iabs(b[0][1] - 2 * b[0][2] + b[0][3]), dq0 = iabs(b[0][4] - 2 * b[0][5] + b[0][6]);
-  const int dp3 = iabs(b[3][1] - 2 * b[3][2] + b[3][3]), dq3 = iabs(b[3][4] - 2 * b[3][5] + b[3][6]);
-  const int dp = dp0 + dp3, dq = dq0 + dq3;
-  if (dp + dq >= beta) return;
-  const bool strong = 2 * (dp0 + dq0) < (beta >> 2) && 2 * (dp3 + dq3) < (beta >> 2) &&
-                      iabs(b[0][3] - b[0][4]) < ((5 * tc + 1) >> 1) && iabs(b[3][3] - b[3][4]) < ((5 * tc + 1) >> 1) &&
-                      iabs(b[0][0] - b[0][3]) + iabs(b[0][4] - b[0][7]) < (beta >> 3) &&
-                      iabs(b[3][0] - b[3][3]) + iabs(b[3][4] - b[3][7]) < (beta >> 3);
-  const int side = (beta + (beta >> 1)) >> 3;
-  for (int l = 0; l < 4; ++l) {
-    const int m0 = b[l][0], m1 = b[l][1], m2 = b[l][2], m3 = b[l][3], m4 = b[l][4], m5 = b[l][5], m6 = b[l][6], m7 = b[l][7];
-    Pix *row = px + l * ys;
-    if (strong) {
-      row[-3 * xs] = (Pix)iclip(m1 - 2 * tc, m1 + 2 * tc, (2 * m0 + 3 * m1 + m2 + m3 + m4 + 4) >> 3);
-      row[-2 * xs] = (Pix)iclip(m2 - 2 * tc, m2 + 2 * tc, (m1 + m2 + m3 + m4 + 2) >> 2);
-      row[-1 * xs] = (Pix)iclip(m3 - 2 * tc, m3 + 2 * tc, (m1 + 2 * m2 + 2 * m3 + 2 * m4 + m5 + 4) >> 3);
-      row[0] = (Pix)iclip(m4 - 2 * tc, m4 + 2 * tc, (m2 + 2 * m3 + 2 * m4 + 2 * m5 + m6 + 4) >> 3);
-      row[xs] = (Pix)iclip(m5 - 2 * tc, m5 + 2 * tc, (m3 + m4 + m5 + m6 + 2) >> 2);
-      row[2 * xs] = (Pix)iclip(m6 - 2 * tc, m6 + 2 * tc, (m3 + m4 + m5 + 3 * m6 + 2 * m7 + 4) >> 3);
-    } else {
-      int delta = (9 * (m4 - m3) - 3 * (m5 - m2) + 8) >> 4;
-      if (iabs(delta) < tc * 10) {
-        delta = iclip(-tc, tc, delta);
-        row[-1 * xs] = (Pix)iclip(0, PixTraits<Pix>::max, m3 + delta);
-        row[0] = (Pix)iclip(0, PixTraits<Pix>::max, m4 - delta);
-        if (dp < side) row[-2 * xs] = (Pix)iclip(0, PixTraits<Pix>::max, m2 + iclip(-(tc >> 1), tc >> 1, (((m1 + m3 + 1) >> 1) - m2 + delta) >> 1));
-        if (dq < side) row[xs] = (Pix)iclip(0, PixTraits<Pix>::max, m5 + iclip(-(tc >> 1), tc >> 1, (((m6 + m4 + 1) >> 1) - m5 - delta) >> 1));
-      }
-    }
-  }
-}
-template <typename Pix> CTU_FN void dbk_chroma_part(Pix *px, int xs, int ys, int tc)      // ref: filter.c:175-192
-{
-  for (int l = 0; l < 4; ++l) {
-    Pix *s = px + l * ys;
-    const int m2 = CTU_LD_FRAME(&s[-2 * xs]), m3 = CTU_LD_FRAME(&s[-xs]), m4 = CTU_LD_FRAME(&s[0]), m5 = CTU_LD_FRAME(&s[xs]);
-    const int delta = iclip(-tc, tc, (((m4 - m3) * 4) + m2 - m5 + 4) >> 3);
-    s[-xs] = (Pix)iclip(0, PixTraits<Pix>::max, m3 + delta);
-    s[0] = (Pix)iclip(0, PixTraits<Pix>::max, m4 - delta);
-  }
-}
+// the deblocking filters (dbk_luma_part, dbk_chroma_part: pixel_rules.h) on the frame planes, read through L2; the luma
+// filter is a call of its own
+struct FrameLoad { template <typename Pix> CTU_MFN int operator()(const Pix *p) const { return CTU_LD_FRAME(p); } };
+template <typename Pix> CTU_FN_NOINLINE void dbk_luma_frame(Pix *px, int xs, int ys, int beta, int tc) { dbk_luma_part<Pix>(px, xs, ys, beta, tc, FrameLoad()); }
+template <typename Pix> CTU_FN void dbk_chroma_frame(Pix *px, int xs, int ys, int tc) { dbk_chroma_part<Pix>(px, xs, ys, tc, FrameLoad()); }
 
 // kvz_filter_deblock_lcu on the frame planes; all CUs are intra (boundary strength 2), fixed QP
 template <typename Pix> CTU_FN_NOINLINE void ctu_deblock(CtuST<Pix> *S, const FrameDevT<Pix> *F, int cx, int cy)
@@ -248,7 +205,7 @@ template <typename Pix> CTU_FN_NOINLINE void ctu_deblock(CtuST<Pix> *S, const Fr
   const int x0 = cx * 64, y0 = cy * 64;
   const int end_x = imin(x0 + 64, Wd), end_y = imin(y0 + 64, H);
   const int qp = cfg->qp;
-  const int scale = 1 << (PixDepth<Pix>::bd - 8);          // bitdepth_scale (ref: filter.c:373, 590)
+  const int scale = 1 << (PixTraits<Pix>::bd - 8);          // bitdepth_scale (ref: filter.c:373, 590)
   const int beta = dbk_beta(iclip(0, 51, qp + 2 * cfg->deblock_beta)) * scale;
   const int tc_l = dbk_tc(iclip(0, 53, qp + 2 + 2 * cfg->deblock_tc)) * scale;
   const int tc_c = dbk_tc(iclip(0, 53, scaled_qp(2, qp, 0) + 2 + 2 * cfg->deblock_tc)) * scale;
@@ -260,10 +217,10 @@ template <typename Pix> CTU_FN_NOINLINE void ctu_deblock(CtuST<Pix> *S, const Fr
     const int ex = x0 + (u % ux_n) * 8, ey = y0 + (u / ux_n) * 8;
     if (ex == 0) continue;
     if (!dbk_edge_wanted(F, ex, ey, false)) continue;
-    if (part < 2) dbk_luma_part(F->rec_y + (size_t)(ey + 4 * part) * Wd + ex, 1, Wd, beta, tc_l);
+    if (part < 2) dbk_luma_frame(F->rec_y + (size_t)(ey + 4 * part) * Wd + ex, 1, Wd, beta, tc_l);
     else if ((ex & 15) == 0) {
-      dbk_chroma_part(F->rec_u + (size_t)(ey / 2) * Wc + ex / 2, 1, Wc, tc_c);
-      dbk_chroma_part(F->rec_v + (size_t)(ey / 2) * Wc + ex / 2, 1, Wc, tc_c);
+      dbk_chroma_frame(F->rec_u + (size_t)(ey / 2) * Wc + ex / 2, 1, Wc, tc_c);
+      dbk_chroma_frame(F->rec_v + (size_t)(ey / 2) * Wc + ex / 2, 1, Wc, tc_c);
     }
   }
   CTU_SYNC();
@@ -279,10 +236,10 @@ template <typename Pix> CTU_FN_NOINLINE void ctu_deblock(CtuST<Pix> *S, const Fr
       const int ey = y0 + it * 8, ex = x0 - 8;          // unit holding the delayed columns
       if (ey == 0) continue;
       if (!dbk_edge_wanted(F, x0 - 4, ey, true)) continue;
-      dbk_luma_part(F->rec_y + (size_t)ey * Wd + x0 - 4, Wd, 1, beta, tc_l);
+      dbk_luma_frame(F->rec_y + (size_t)ey * Wd + x0 - 4, Wd, 1, beta, tc_l);
       if ((ey & 15) == 0) {
-        dbk_chroma_part(F->rec_u + (size_t)(ey / 2) * Wc + x0 / 2 - 4, Wc, 1, tc_c);
-        dbk_chroma_part(F->rec_v + (size_t)(ey / 2) * Wc + x0 / 2 - 4, Wc, 1, tc_c);
+        dbk_chroma_frame(F->rec_u + (size_t)(ey / 2) * Wc + x0 / 2 - 4, Wc, 1, tc_c);
+        dbk_chroma_frame(F->rec_v + (size_t)(ey / 2) * Wc + x0 / 2 - 4, Wc, 1, tc_c);
       }
       (void)ex;
       continue;
@@ -293,11 +250,11 @@ template <typename Pix> CTU_FN_NOINLINE void ctu_deblock(CtuST<Pix> *S, const Fr
     if (ey == 0) continue;
     if (!dbk_edge_wanted(F, ex, ey, true)) continue;
     const bool delayed = ((ex + 8) % 64 == 0) && (ex + 8 != Wd);
-    if (part == 0) dbk_luma_part(F->rec_y + (size_t)ey * Wd + ex, Wd, 1, beta, tc_l);
-    else if (part == 1) { if (!delayed) dbk_luma_part(F->rec_y + (size_t)ey * Wd + ex + 4, Wd, 1, beta, tc_l); }
+    if (part == 0) dbk_luma_frame(F->rec_y + (size_t)ey * Wd + ex, Wd, 1, beta, tc_l);
+    else if (part == 1) { if (!delayed) dbk_luma_frame(F->rec_y + (size_t)ey * Wd + ex + 4, Wd, 1, beta, tc_l); }
     else if ((ey & 15) == 0 && !delayed) {
-      dbk_chroma_part(F->rec_u + (size_t)(ey / 2) * Wc + ex / 2, Wc, 1, tc_c);
-      dbk_chroma_part(F->rec_v + (size_t)(ey / 2) * Wc + ex / 2, Wc, 1, tc_c);
+      dbk_chroma_frame(F->rec_u + (size_t)(ey / 2) * Wc + ex / 2, Wc, 1, tc_c);
+      dbk_chroma_frame(F->rec_v + (size_t)(ey / 2) * Wc + ex / 2, Wc, 1, tc_c);
     }
   }
   CTU_SYNC();
@@ -309,19 +266,12 @@ struct SaoStats {
   int32_t band[3][2][32];       // [plane][sum, count][band]
 };
 
-CTU_FN int sao_eo_cat(int a, int b, int cc)
-{
-  const int map[5] = { 1, 2, 0, 3, 4 };
-  const int s1 = cc > a ? 1 : (cc < a ? -1 : 0), s2 = cc > b ? 1 : (cc < b ? -1 : 0);
-  return map[2 + s1 + s2];
-}
-
 // statistics of the CTU's block of one plane (the reference works on a contiguous copy: same pixels)
 template <typename Pix> CTU_FN_NOINLINE void sao_stats_plane(const Pix *org, const Pix *rec, int stride, int bw, int bh, int32_t edge[4][2][5], int32_t band[2][32])
 {
   // bands: the top five bits of the sample (ref: sao.c:273); edge sums: differences rounded to 8-bit precision
   // (ref: sao-generic.c:66-77)
-  constexpr int band_shift = PixDepth<Pix>::bd - 5, edge_shift = PixDepth<Pix>::bd - 8;
+  constexpr int band_shift = PixTraits<Pix>::bd - 5, edge_shift = PixTraits<Pix>::bd - 8;
   constexpr int edge_round = edge_shift ? 1 << (edge_shift - 1) : 0;
   #pragma unroll 1
   for (int e = CTU_TID; e < bw * bh; e += CTU_NT) {
@@ -330,9 +280,10 @@ template <typename Pix> CTU_FN_NOINLINE void sao_stats_plane(const Pix *org, con
     CTU_ATOMIC_ADD(&band[0][cc >> band_shift], d);
     CTU_ATOMIC_ADD(&band[1][cc >> band_shift], 1);
     if (x >= 1 && x < bw - 1 && y >= 1 && y < bh - 1) {
-      const int ax[4] = { -1, 0, -1, 1 }, ay[4] = { 0, -1, -1, -1 };
       for (int k = 0; k < 4; ++k) {
-        const int a = CTU_LD_FRAME(&rec[(y + ay[k]) * stride + x + ax[k]]), b = CTU_LD_FRAME(&rec[(y - ay[k]) * stride + x - ax[k]]);
+        int ax, ay;
+        sao_eo_offsets(k, ax, ay);
+        const int a = CTU_LD_FRAME(&rec[(y + ay) * stride + x + ax]), b = CTU_LD_FRAME(&rec[(y - ay) * stride + x - ax]);
         const int cat = sao_eo_cat(a, b, cc);
         CTU_ATOMIC_ADD(&edge[k][0][cat], (d + edge_round) >> edge_shift);
         CTU_ATOMIC_ADD(&edge[k][1][cat], 1);
@@ -735,22 +686,18 @@ template <typename Pix> CTU_FN_NOINLINE void ctu_sao_apply(const CtuConfig *cfg,
     const int bw = imin(64 >> sh, pw - x0), bh = imin(64 >> sh, ph - y0);
     const int type = cfg->sao_type ? s->type : 0;
     const int ov = plane == 2 ? 5 : 0;
-    const int ax[4] = { -1, 0, -1, 1 }, ay[4] = { 0, -1, -1, -1 };
     #pragma unroll 1
     for (int e = CTU_TID; e < bw * bh; e += CTU_NT) {
       const int y = y0 + e / bw, x = x0 + e % bw;
       const int cc = in[(size_t)y * pw + x];
       int v = cc;
-      if (type == 1) {
-        const int k = (cc >> (PixDepth<Pix>::bd - 5)) - s->band_position[plane == 2 ? 1 : 0];
-        if (k >= 0 && k <= 3) v = iclip(0, PixTraits<Pix>::max, cc + s->offsets[k + 1 + ov]);
-      } else if (type == 2) {
-        const int dx = ax[s->eo_class], dy = ay[s->eo_class];
+      if (type == 1) v = sao_band_px(cc, PixTraits<Pix>::bd, s->band_position[plane == 2 ? 1 : 0], s->offsets + ov);
+      else if (type == 2) {
+        int dx, dy;
+        sao_eo_offsets(s->eo_class, dx, dy);
         const int xa = x + dx, ya = y + dy, xb = x - dx, yb = y - dy;
-        if (xa >= 0 && xa < pw && xb >= 0 && xb < pw && ya >= 0 && ya < ph && yb >= 0 && yb < ph) {
-          const int cat = sao_eo_cat(in[(size_t)ya * pw + xa], in[(size_t)yb * pw + xb], cc);
-          v = iclip(0, PixTraits<Pix>::max, cc + s->offsets[cat + ov]);
-        }
+        if (xa >= 0 && xa < pw && xb >= 0 && xb < pw && ya >= 0 && ya < ph && yb >= 0 && yb < ph)
+          v = sao_edge_px(cc, in[(size_t)ya * pw + xa], in[(size_t)yb * pw + xb], PixTraits<Pix>::bd, s->offsets + ov);
       }
       out[(size_t)y * pw + x] = (Pix)v;
     }

@@ -1,7 +1,8 @@
 // ctu_leaf.h -- block-level operations of the CTU search driver, written for the execution model of ctu_common.h
 // (every function is called by all threads of the CTA unless it says "leader only" / "team").
 //
-// Reference semantics restated here (8- and 10-bit, 4:2:0, flat scaling lists):
+// Reference semantics (8- and 10-bit, 4:2:0, flat scaling lists); the rules shared with the strategy kernels are in
+// pixel_rules.h (prediction, smoothing, availability) and coeff_rules.h (quantisation and coefficient coding):
 //   intra references     src/intra.c:305-559 (kvz_intra_build_reference_any / _inner), :176-204 (smoothing)
 //   intra prediction     src/intra.c:252-302 + strategies/generic/intra-generic.c:49-241
 //   SATD / SAD           strategies/generic/picture-generic.c:117-340, 475-501
@@ -201,22 +202,12 @@ template <typename Pix> CTU_FN void refs_smooth_dc_p(int l2p, int mask, int n0, 
   for (int i = CTU_TID; i < 2 * n0 + 3; i += CTU_NT) {
     if (i >= 2 * n0) {
       const int color = i - 2 * n0;
-      if ((mask >> color) & 1) {
-        const int w = 1 << log2w_of(l2p, color);
-        int s = 0;
-        for (int k = 1; k <= w; ++k) s += r[color].top[k] + r[color].left[k];
-        r[color].dc = (s + w) >> (log2w_of(l2p, color) + 1);
-      }
+      if ((mask >> color) & 1) r[color].dc = dc_value(log2w_of(l2p, color), r[color].top, r[color].left);
       continue;
     }
     const bool is_top = i >= n0;
     const int e = is_top ? i - n0 : i;
-    const Pix *p = is_top ? r[0].top : r[0].left;
-    int v;
-    if (e == 0) v = (r[0].left[1] + 2 * r[0].left[0] + r[0].top[1] + 2) >> 2;
-    else if (e == n0 - 1) v = p[e];
-    else v = (p[e - 1] + 2 * p[e] + p[e + 1] + 2) >> 2;
-    (is_top ? r[0].ftop : r[0].fleft)[e] = (Pix)v;
+    (is_top ? r[0].ftop : r[0].fleft)[e] = (Pix)ref_smooth_entry(r[0].top, r[0].left, is_top, e, n0);
   }
   CTU_SYNC();
 }
@@ -235,7 +226,7 @@ template <typename Pix> CTU_FN_NOINLINE void build_refs_multi(const SmTables *T0
   IntraRefs<Pix> *r = sm(r0);
   const int lx = x & 63, ly = y & 63;
   const bool has_left = x > 0, has_top = y > 0, inner = has_left && has_top;
-  const int mid = 1 << (PixDepth<Pix>::bd - 1);       // value of unavailable references (ref: intra.c:319)
+  const int mid = 1 << (PixTraits<Pix>::bd - 1);       // value of unavailable references (ref: intra.c:319)
   int n_of[3], start[4];
   start[0] = 0;
   for (int col = 0; col < 3; ++col) { n_of[col] = ((mask >> col) & 1) ? 2 * (1 << log2w_of(l2p, col)) + 1 : 0; start[col + 1] = start[col] + 2 * n_of[col]; }
@@ -247,11 +238,9 @@ template <typename Pix> CTU_FN_NOINLINE void build_refs_multi(const SmTables *T0
     const Plane<Pix> P = plane_of(W, L, color);
     const int px = lx >> is_c, py = ly >> is_c, lw = P.lw;
     int al = 0, at = 0;
-    if (has_left) { al = T->ref_left[ly >> 2][lx >> 2] >> is_c; al = imin(al, 2 * w); al = imin(al, (height - y) >> is_c); }
-    if (has_top) { at = T->ref_top[ly >> 2][lx >> 2] >> is_c; at = imin(at, 2 * w); at = imin(at, (width - x) >> is_c); }
-    // the _inner variant copies in groups of four, at least one group (intra.c:486-494, 512-516)
-    const int nl = inner ? imax(4, (al + 3) & ~3) : al;
-    const int ntp = inner ? imax(4, (at + 3) & ~3) : at;
+    if (has_left) al = ref_avail(T->ref_left[ly >> 2][lx >> 2], is_c, w, height - y);
+    if (has_top) at = ref_avail(T->ref_top[ly >> 2][lx >> 2], is_c, w, width - x);
+    const int nl = ref_copied(inner, al), ntp = ref_copied(inner, at);
     // border accessors: k >= -1
 #define CTU_TOP_BORDER(k) (py ? P.rec[(px + (k)) + (py - 1) * lw] : P.top[1 + px + (k)])
 #define CTU_LEFT_BORDER(k) (px ? P.rec[(px - 1) + (py + (k)) * lw] : P.left[1 + py + (k)])
@@ -281,77 +270,8 @@ template <typename Pix> CTU_FN void build_refs(const SmTables *T, const CtuConfi
 }
 
 // ------------------------------------------------------------------------------------------------ intra prediction
-// The sample displacement and its inverse for an angular mode at |mode - 26| (vertical) / |10 - mode| (horizontal) =
-// adisp, 0..8 (modedisp2sampledisp, modedisp2invsampledisp: intra-generic.c:59-60), as immediates packed into 64-bit
-// words: a 9-entry array indexed at run time would be built in local memory on every use, inside the per-sample loops.
-CTU_FN int ang_disp(int adisp)          // 0, 2, 5, 9, 13, 17, 21, 26, 32
-{
-  return adisp == 8 ? 32 : (int)((0x1A15110D09050200ull >> (8 * adisp)) & 0xff);
-}
-CTU_FN int ang_inv(int adisp)           // 0, 4096, 1638, 910, 630, 482, 390, 315, 256
-{
-  if (adisp == 8) return 256;
-  const uint64_t w = adisp < 4 ? 0x038E066610000000ull : 0x013B018601E20276ull;
-  return (int)((w >> (16 * (adisp & 3))) & 0xffff);
-}
-template <typename Pix> CTU_FN int ang_ref(const Pix *rmain, const Pix *rside, int idx, int inv)
-{
-  if (idx >= -1) return rmain[idx + 1];
-  const int k = -idx - 1;
-  return rside[(128 + k * inv) >> 8];
-}
-template <typename Pix> CTU_FN int angular_px(int mode, const Pix *top, const Pix *left, int ox, int oy)
-{
-  const bool vertical = mode >= 18;
-  const int mdisp = vertical ? mode - 26 : 10 - mode;
-  const int adisp = iabs(mdisp);
-  const int sdisp = mdisp < 0 ? -ang_disp(adisp) : ang_disp(adisp);
-  const Pix *rmain = vertical ? top : left;
-  const Pix *rside = vertical ? left : top;
-  const int x = vertical ? ox : oy, y = vertical ? oy : ox;
-  if (sdisp == 0) return rmain[x + 1];
-  const int pos = (y + 1) * sdisp;
-  const int di = pos >> 5, df = pos & 31;
-  const int inv = ang_inv(adisp);
-  const int r1 = ang_ref(rmain, rside, x + di, inv);
-  if (df == 0) return r1;
-  const int r2 = ang_ref(rmain, rside, x + di + 1, inv);
-  return ((32 - df) * r1 + df * r2 + 16) >> 5;
-}
-CTU_FN bool intra_uses_filtered(int log2w, int mode, int color)
-{
-  if (color != 0 || mode == 1 || log2w == 2) return false;
-  if (mode == 0) return true;
-  const int thres = log2w == 3 ? 7 : (log2w == 4 ? 1 : 0);
-  return imin(iabs(mode - 26), iabs(mode - 10)) > thres;
-}
-// kvz_intra_predict for one sample (filter_boundary is always true: no lossless / implicit RDPCM)
-template <typename Pix> CTU_FN int intra_predict_px(const IntraRefs<Pix> *r, int log2w, int mode, int color, int x, int y)
-{
-  const bool f = intra_uses_filtered(log2w, mode, color);
-  const Pix *t = f ? r->ftop : r->top, *l = f ? r->fleft : r->left;
-  const int w = 1 << log2w;
-  if (mode == 0) {
-    const int hor = (w - 1 - x) * l[y + 1] + (x + 1) * t[w + 1];
-    const int ver = (w - 1 - y) * t[x + 1] + (y + 1) * l[w + 1];
-    return (ver + hor + w) >> (log2w + 1);
-  }
-  if (mode == 1) {
-    const int dc = r->dc;
-    if (color == 0 && log2w < 5) {
-      if (x == 0 && y == 0) return (l[1] + 2 * dc + t[1] + 2) >> 2;
-      if (y == 0) return (t[x + 1] + 3 * dc + 2) >> 2;
-      if (x == 0) return (l[y + 1] + 3 * dc + 2) >> 2;
-    }
-    return dc;
-  }
-  int v = angular_px(mode, t, l, x, y);
-  if (color == 0 && log2w < 5) {
-    if (mode == 10 && y == 0) v = iclip(0, PixTraits<Pix>::max, v + ((t[x + 1] - t[0]) >> 1));
-    else if (mode == 26 && x == 0) v = iclip(0, PixTraits<Pix>::max, v + ((l[y + 1] - l[0]) >> 1));
-  }
-  return v;
-}
+// (the rules: intra_predict_px and what it calls, pixel_rules.h; filter_boundary is always true here: no lossless /
+// implicit RDPCM)
 // prediction of a whole block into dst (row stride dst_stride)
 template <typename Pix> CTU_FN_NOINLINE void predict_block(const IntraRefs<Pix> *r, int log2w, int mode, int color, Pix *dst, int dst_stride)
 {
@@ -359,7 +279,7 @@ template <typename Pix> CTU_FN_NOINLINE void predict_block(const IntraRefs<Pix> 
   #pragma unroll 1
   for (int e = CTU_TID; e < w * w; e += CTU_NT) {
     const int y = e >> log2w, x = e & (w - 1);
-    dst[y * dst_stride + x] = (Pix)intra_predict_px(r, log2w, mode, color, x, y);
+    dst[y * dst_stride + x] = (Pix)intra_predict_px<Pix>(*r, log2w, mode, color, true, x, y);
   }
   CTU_SYNC();
 }
@@ -444,7 +364,7 @@ CTU_FN void rough_diff_block(const IntraRefs<Pix> *r, const RoughExt<Pix> *ext, 
 #pragma unroll
       for (int x = 0; x < W8; ++x) {
         int v = ((32 - df) * (int)p[x] + df * (int)p[x + 1] + 16) >> 5;
-        if (edge && x == 0) v = iclip(0, PixTraits<Pix>::max, v + (((int)side[oy + y + 1] - (int)side[0]) >> 1));
+        if (edge && x == 0) v = intra_edge_px<Pix>(v, side[oy + y + 1], side[0]);
         d[y * W8 + x] = v - (int)src[(oy + y) * sy + (ox + x) * sx];
       }
     }
@@ -522,10 +442,10 @@ template <typename Pix> CTU_FN_NOINLINE void rough_costs_all_modes(const IntraRe
     }
   }
   CTU_SYNC();
-  if constexpr (PixDepth<Pix>::bd != 8) {
+  if constexpr (PixTraits<Pix>::bd != 8) {
     // above 8 bits the reference's SATD of 8x8 and larger blocks and its SAD are scaled to 8-bit precision
     // (strategies-picture.h:68, picture-generic.c:381, 484, 521); the 4x4 SATD is not
-    constexpr int sh = PixDepth<Pix>::bd - 8;
+    constexpr int sh = PixTraits<Pix>::bd - 8;
     #pragma unroll 1
     for (int m = CTU_TID; m < 35; m += CTU_NT) { if (w > 4) satd_out[m] >>= sh; sad_out[m] >>= sh; }
     CTU_SYNC();
@@ -611,38 +531,6 @@ CTU_FN int ilog2(int n) { int l = 0; while ((1 << l) < n) ++l; return l; }
 
 // ------------------------------------------------------------------------------------------------ quantisation
 
-// sign-bit hiding of kvz_quant for one coefficient group (ref: quant-generic.c:84-176)
-CTU_FN void quant_sign_hide_group(const SmTables *T, const int16_t *coef, int16_t *q, const int32_t *delta_u, const int32_t *cg_nz,
-                                  int num_cg, int g, int scan_idx, int log2n)
-{
-  bool last_cg = true;
-  for (int h = g + 1; h < num_cg; ++h) if (cg_nz[h]) { last_cg = false; break; }
-  const uint16_t *pos = &sm_scan(T, scan_idx, log2n - 2)[g * 16];
-  int first_nz = 16, last_nz = -1, abssum = 0;
-  for (int k = 15; k >= 0; --k) if (q[pos[k]]) { last_nz = k; break; }
-  for (int k = 0; k < 16; ++k) if (q[pos[k]]) { first_nz = k; break; }
-  for (int k = first_nz; k <= last_nz; ++k) abssum += q[pos[k]];
-  if (last_nz - first_nz < 4) return;
-  const int signbit = q[pos[first_nz]] > 0 ? 0 : 1;
-  if (signbit == (abssum & 1)) return;
-  int min_cost = 0x7fffffff, cur_cost = 0x7fffffff, min_pos = -1;
-  int final_change = 0, cur_change = 0;
-  for (int k = (last_cg ? last_nz : 15); k >= 0; --k) {
-    const int b = pos[k];
-    if (q[b] != 0) {
-      if (delta_u[b] > 0) { cur_cost = -delta_u[b]; cur_change = 1; }
-      else if (k == first_nz && iabs((int)q[b]) == 1) { cur_cost = 0x7fffffff; }
-      else { cur_cost = delta_u[b]; cur_change = -1; }
-    } else if (k < first_nz && ((coef[b] >= 0) ? 0 : 1) != signbit) {
-      cur_cost = 0x7fffffff;
-    } else { cur_cost = -delta_u[b]; cur_change = 1; }
-    if (cur_cost < min_cost) { min_cost = cur_cost; final_change = cur_change; min_pos = b; }
-  }
-  if (q[min_pos] == 32767 || q[min_pos] == -32768) final_change = -1;
-  if (coef[min_pos] >= 0) q[min_pos] = (int16_t)(q[min_pos] + final_change);
-  else q[min_pos] = (int16_t)(q[min_pos] - final_change);
-}
-
 // kvz_quant: b -> q (intra slice: rounding offset 171)
 template <typename Pix> CTU_FN_NOINLINE void quant_block(Team tm, const SmTables *T0, int qp, bool signhide, TuS<Pix> tu, int n, int type, int scan_idx)
 {
@@ -651,7 +539,7 @@ template <typename Pix> CTU_FN_NOINLINE void quant_block(Team tm, const SmTables
   const int log2n = ilog2(n);
   const int qp_scaled = scaled_qp_px<Pix>(type, qp);
   const int qc = quant_scale(qp_scaled % 6);
-  const int transform_shift = 15 - PixDepth<Pix>::bd - log2n;
+  const int transform_shift = 15 - PixTraits<Pix>::bd - log2n;
   const int q_bits = 14 + qp_scaled / 6 + transform_shift;
   const int add = 171 << (q_bits - 9);
   const int q_bits8 = q_bits - 8;
@@ -685,7 +573,7 @@ template <typename Pix> CTU_FN_NOINLINE void quant_block(Team tm, const SmTables
   tsync(tm);
   #pragma unroll 1
   for (int g = tm.tid; g < num_cg; g += tm.nt)
-    if (cg_nz[g]) quant_sign_hide_group(T, b, q, d, cg_nz, num_cg, g, scan_idx, log2n);
+    if (cg_nz[g]) quant_sign_hiding(&sm_scan(T, scan_idx, log2n - 2)[g * 16], b, q, d, cg_nz, num_cg, g);
   tsync(tm);
 }
 
@@ -695,7 +583,7 @@ CTU_FN_NOINLINE void dequant_block(Team tm, int qp, TuS<Pix> tu, int n_rt, int t
 {
   tu.base = sm(tu.base);
   const int n = L2N ? (1 << L2N) : n_rt;
-  const int transform_shift = 15 - PixDepth<Pix>::bd - (L2N ? L2N : ilog2(n));
+  const int transform_shift = 15 - PixTraits<Pix>::bd - (L2N ? L2N : ilog2(n));
   const int qp_scaled = scaled_qp_px<Pix>(type, qp);
   const int shift = 20 - 14 - transform_shift;
   const int scale = inv_quant_scale(qp_scaled % 6) << (qp_scaled / 6);
@@ -713,7 +601,7 @@ CTU_FN_NOINLINE void dequant_block(Team tm, int qp, TuS<Pix> tu, int n_rt, int t
 template <typename Pix> CTU_FN_NOINLINE void rdoq_sign_hiding(TuS<Pix> tu, const uint16_t *blk, double lambda, int qp_scaled, int last_pos, const int16_t *coef, int16_t *q)
 {
   tu.base = sm(tu.base);
-  kvzcoeff::rdoq_sign_hiding(tu.inc(), tu.dec(), tu.sig_inc(), tu.qdelta(), sm(blk), lambda, PixDepth<Pix>::bd, qp_scaled, last_pos, sm(coef), sm(q));
+  kvzcoeff::rdoq_sign_hiding(tu.inc(), tu.dec(), tu.sig_inc(), tu.qdelta(), sm(blk), lambda, PixTraits<Pix>::bd, qp_scaled, last_pos, sm(coef), sm(q));
 }
 
 // RDOQ runs on the first nl = rdoq_lanes() threads of a team (the first warp of a CTA team), whose lanes are `mask`
@@ -746,7 +634,7 @@ CTU_FN_NOINLINE void rdoq_team(const SmTables *T0, const uint8_t *cabac0, int qp
   int32_t *s_inc = tu.inc(), *s_dec = tu.dec(), *s_sig_inc = tu.sig_inc(), *s_qdelta = tu.qdelta(), *s_cg_flag = tu.cg_flag();
   uint16_t *s_cg_nz = tu.cg_nz();
   const int n = 1 << log2n, nn = n * n;
-  const int transform_shift = 15 - PixDepth<Pix>::bd - log2n;
+  const int transform_shift = 15 - PixTraits<Pix>::bd - log2n;
   const int qp_scaled = scaled_qp_px<Pix>(type, qp);
   const int q_bits = 14 + qp_scaled / 6 + transform_shift;
   const int qc = quant_scale(qp_scaled % 6);
@@ -755,7 +643,7 @@ CTU_FN_NOINLINE void rdoq_team(const SmTables *T0, const uint8_t *cabac0, int qp
   double err_scale = 32768.0;
   for (int i = 0; i < 2 * transform_shift; ++i) err_scale *= 0.5;
   for (int i = 0; i > 2 * transform_shift; --i) err_scale *= 2.0;
-  err_scale = err_scale / qc / qc / (1 << (2 * (PixDepth<Pix>::bd - 8)));
+  err_scale = err_scale / qc / qc / (1 << (2 * (PixTraits<Pix>::bd - 8)));
   const RdoqModels m = rdoq_models(cabac, T->ebits, type);
   auto sig_cost_of = [&](uint8_t code) { return (code >> 6) == 2 ? 0.0 : lambda * ebits(m, m.sig[code & 63], code >> 6); };
   auto level0_cost = [&](int blk) { const double e = (double)imin(iabs((int)coef[blk]) * qc, 0x7FFFFFFF - half); return e * e * err_scale; };
@@ -1070,14 +958,14 @@ CTU_FN_NOINLINE void tu_core_t(Team tm, const SmTables *T0, const CtuConfig *cfg
   j.refs = sm(j.refs);
   const int log2n = L2N ? L2N : j.log2n, n = 1 << log2n, nn = n * n;
   const int color = j.color;
-  const int ts_shift = 15 - PixDepth<Pix>::bd - log2n;
+  const int ts_shift = 15 - PixTraits<Pix>::bd - log2n;
   int16_t *a = tu.a(), *b = tu.b(), *q = tu.q(), *t = tu.t();
   Pix *pred = tu.pred(), *rec = tu.rec();
   TuFixed<Pix> *fx = tu.fx();
   #pragma unroll 1
   for (int e = tm.tid; e < nn; e += tm.nt) {
     const int y = e >> log2n, x = e & (n - 1);
-    const int p = intra_predict_px(j.refs, log2n, j.mode, color, x, y);
+    const int p = intra_predict_px<Pix>(*j.refs, log2n, j.mode, color, true, x, y);
     pred[e] = (Pix)p;
     a[e] = (int16_t)((int)j.src[y * j.src_stride + x] - p);
   }
@@ -1090,7 +978,7 @@ CTU_FN_NOINLINE void tu_core_t(Team tm, const SmTables *T0, const CtuConfig *cfg
     for (int e = tm.tid; e < nn; e += tm.nt) b[e] = (int16_t)((uint16_t)a[e] << ts_shift);
     tsync(tm);
   } else {
-    fwd_pass<L2N>(tm, a, t, M, n, log2n - 1 + (PixDepth<Pix>::bd - 8));
+    fwd_pass<L2N>(tm, a, t, M, n, log2n - 1 + (PixTraits<Pix>::bd - 8));
     fwd_pass<L2N>(tm, t, b, M, n, log2n + 6);
   }
   const int type = color == 0 ? 0 : 2;
@@ -1126,7 +1014,7 @@ CTU_FN_NOINLINE void tu_core_t(Team tm, const SmTables *T0, const CtuConfig *cfg
       tsync(tm);
     } else {
       inv_pass<L2N>(tm, b, t, M, n, 7);
-      inv_pass<L2N>(tm, t, a, M, n, 12 - (PixDepth<Pix>::bd - 8));
+      inv_pass<L2N>(tm, t, a, M, n, 12 - (PixTraits<Pix>::bd - 8));
     }
     #pragma unroll 1
     for (int e = tm.tid; e < nn; e += tm.nt) {
@@ -1149,9 +1037,9 @@ CTU_FN_NOINLINE void tu_core_t(Team tm, const SmTables *T0, const CtuConfig *cfg
   }
   if (ssd) CTU_ATOMIC_ADD(&fx->ssd, ssd);
   tsync(tm);
-  if constexpr (PixDepth<Pix>::bd != 8) {
+  if constexpr (PixTraits<Pix>::bd != 8) {
     // kvz_pixels_calc_ssd scales the unit's SSD to 8-bit precision (picture-generic.c:550)
-    if (tm.tid == 0) fx->ssd >>= 2 * (PixDepth<Pix>::bd - 8);
+    if (tm.tid == 0) fx->ssd >>= 2 * (PixTraits<Pix>::bd - 8);
     tsync(tm);
   }
 }

@@ -15,15 +15,7 @@
 
 namespace kvzc {
 
-__constant__ uint8_t c_dbk_tc[54] = { 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 1, 1, 1, 1, 1, 1, 1, 1, 1, 2, 2, 2, 2, 3, 3, 3, 3, 4, 4,
-                                      4, 5, 5, 6, 6, 7, 8, 9, 10, 11, 13, 14, 16, 18, 20, 22, 24 };
-__device__ __forceinline__ int dbk_beta(int i) { return i < 16 ? 0 : (i < 29 ? i - 10 : 2 * i - 38); }
-__device__ __forceinline__ int dbk_chroma_qp(int qp)
-{
-  // kvz_g_chroma_scale (transform.c:56-62): identity below 30, qp - 6 from 44, the HEVC table between
-  const int mid[14] = { 29, 30, 31, 32, 33, 33, 34, 34, 35, 35, 36, 36, 37, 37 };
-  return qp < 30 ? qp : (qp < 44 ? mid[qp - 30] : qp - 6);
-}
+__constant__ uint8_t c_dbk_tc[54] = { PIX_DBK_TC };
 
 struct DbkCu {
   uint32_t w0, w1, mv0, mv1, w4;
@@ -95,63 +87,6 @@ __device__ __forceinline__ int dbk_qp(const kvz_cuda_dbk_params &p, const uint32
   return (qp_p + dbk_cu_at(cus, p.cu_stride_scu, x, y).qp() + 1) >> 1;
 }
 
-// luma part: px -> q0 of line 0; xs across the edge, ys along it  (filter.c:95-170, 474-520)
-template <class T>
-__device__ __forceinline__ void dbk_luma_part(T *px, long xs, long ys, int beta, int tc)
-{
-  constexpr int PIXMAX = (1 << PixTraits<T>::kBits) - 1;
-  int b[4][8];
-#pragma unroll
-  for (int l = 0; l < 4; ++l)
-#pragma unroll
-    for (int i = 0; i < 8; ++i) b[l][i] = px[l * ys + (i - 4) * xs];
-  const int dp0 = abs(b[0][1] - 2 * b[0][2] + b[0][3]), dq0 = abs(b[0][4] - 2 * b[0][5] + b[0][6]);
-  const int dp3 = abs(b[3][1] - 2 * b[3][2] + b[3][3]), dq3 = abs(b[3][4] - 2 * b[3][5] + b[3][6]);
-  const int dp = dp0 + dp3, dq = dq0 + dq3;
-  if (dp + dq >= beta) return;
-  const bool strong = 2 * (dp0 + dq0) < (beta >> 2) && 2 * (dp3 + dq3) < (beta >> 2) &&
-                      abs(b[0][3] - b[0][4]) < ((5 * tc + 1) >> 1) && abs(b[3][3] - b[3][4]) < ((5 * tc + 1) >> 1) &&
-                      abs(b[0][0] - b[0][3]) + abs(b[0][4] - b[0][7]) < (beta >> 3) &&
-                      abs(b[3][0] - b[3][3]) + abs(b[3][4] - b[3][7]) < (beta >> 3);
-  const int side = (beta + (beta >> 1)) >> 3;
-#pragma unroll
-  for (int l = 0; l < 4; ++l) {
-    const int m0 = b[l][0], m1 = b[l][1], m2 = b[l][2], m3 = b[l][3], m4 = b[l][4], m5 = b[l][5], m6 = b[l][6], m7 = b[l][7];
-    T *row = px + l * ys;
-    if (strong) {
-      row[-3 * xs] = (T)clip3(m1 - 2 * tc, m1 + 2 * tc, (2 * m0 + 3 * m1 + m2 + m3 + m4 + 4) >> 3);
-      row[-2 * xs] = (T)clip3(m2 - 2 * tc, m2 + 2 * tc, (m1 + m2 + m3 + m4 + 2) >> 2);
-      row[-1 * xs] = (T)clip3(m3 - 2 * tc, m3 + 2 * tc, (m1 + 2 * m2 + 2 * m3 + 2 * m4 + m5 + 4) >> 3);
-      row[0] = (T)clip3(m4 - 2 * tc, m4 + 2 * tc, (m2 + 2 * m3 + 2 * m4 + 2 * m5 + m6 + 4) >> 3);
-      row[xs] = (T)clip3(m5 - 2 * tc, m5 + 2 * tc, (m3 + m4 + m5 + m6 + 2) >> 2);
-      row[2 * xs] = (T)clip3(m6 - 2 * tc, m6 + 2 * tc, (m3 + m4 + m5 + 3 * m6 + 2 * m7 + 4) >> 3);
-    } else {
-      int delta = (9 * (m4 - m3) - 3 * (m5 - m2) + 8) >> 4;
-      if (abs(delta) < tc * 10) {
-        delta = clip3(-tc, tc, delta);
-        row[-1 * xs] = (T)clip3(0, PIXMAX, m3 + delta);
-        row[0] = (T)clip3(0, PIXMAX, m4 - delta);
-        if (dp < side) row[-2 * xs] = (T)clip3(0, PIXMAX, m2 + clip3(-(tc >> 1), tc >> 1, (((m1 + m3 + 1) >> 1) - m2 + delta) >> 1));
-        if (dq < side) row[xs] = (T)clip3(0, PIXMAX, m5 + clip3(-(tc >> 1), tc >> 1, (((m6 + m4 + 1) >> 1) - m5 - delta) >> 1));
-      }
-    }
-  }
-}
-
-template <class T>
-__device__ __forceinline__ void dbk_chroma_part(T *px, long xs, long ys, int tc)      // filter.c:175-192
-{
-  constexpr int PIXMAX = (1 << PixTraits<T>::kBits) - 1;
-#pragma unroll
-  for (int l = 0; l < 4; ++l) {
-    T *s = px + l * ys;
-    const int m2 = s[-2 * xs], m3 = s[-xs], m4 = s[0], m5 = s[xs];
-    const int delta = clip3(-tc, tc, (((m4 - m3) * 4) + m2 - m5 + 4) >> 3);
-    s[-xs] = (T)clip3(0, PIXMAX, m3 + delta);
-    s[0] = (T)clip3(0, PIXMAX, m4 - delta);
-  }
-}
-
 // One pass (HOR = false: vertical edges, true: horizontal edges).  blockIdx.y = plane.
 //   luma   : parts indexed (along-edge 4-sample index, edge index); thread order follows the sample rows
 //   chroma : one part per 8x8 luma unit whose edge coordinate is a multiple of 16
@@ -160,7 +95,7 @@ __global__ void __launch_bounds__(128) deblock_pass_kernel(kvz_cuda_dbk_params p
                                                            const uint32_t *__restrict__ cus)
 {
   const int W = p.width, H = p.height;
-  const int scale = 1 << (PixTraits<T>::kBits - 8);
+  const int scale = 1 << (PixTraits<T>::bd - 8);
   const int plane = blockIdx.y;
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
   if (plane == 0) {
@@ -178,7 +113,7 @@ __global__ void __launch_bounds__(128) deblock_pass_kernel(kvz_cuda_dbk_params p
     const int qp = dbk_qp(p, cus, ux, uy, HOR);
     const int beta = dbk_beta(clip3(0, 51, qp + 2 * p.beta_offset_div2)) * scale;
     const int tc = c_dbk_tc[clip3(0, 53, qp + 2 * (bs - 1) + 2 * p.tc_offset_div2)] * scale;
-    dbk_luma_part<T>(y + (size_t)py * W + px, HOR ? W : 1, HOR ? 1 : W, beta, tc);
+    dbk_luma_part<T, long>(y + (size_t)py * W + px, HOR ? W : 1, HOR ? 1 : W, beta, tc);
   } else {
     if (!u || !v) return;
     const int Wc = W / 2, Hc = H / 2;
@@ -193,10 +128,10 @@ __global__ void __launch_bounds__(128) deblock_pass_kernel(kvz_cuda_dbk_params p
     if (!dbk_edge_wanted(cus, p.cu_stride_scu, ex, ey, HOR, tu_boundary)) return;
     const int cx = ex / 2, cy = ey / 2;
     if (cx >= Wc || cy >= Hc) return;
-    const int qpc = dbk_chroma_qp(dbk_qp(p, cus, ex, ey, HOR));
+    const int qpc = kvzcoeff::scaled_qp(2, dbk_qp(p, cus, ex, ey, HOR), 0);       // kvz_g_chroma_scale (filter.c:589)
     const int tc = c_dbk_tc[clip3(0, 53, qpc + 2 + 2 * p.tc_offset_div2)] * scale;
     T *pl = plane == 1 ? u : v;
-    dbk_chroma_part<T>(pl + (size_t)cy * Wc + cx, HOR ? Wc : 1, HOR ? 1 : Wc, tc);
+    dbk_chroma_part<T, long>(pl + (size_t)cy * Wc + cx, HOR ? Wc : 1, HOR ? 1 : Wc, tc);
   }
 }
 

@@ -49,7 +49,7 @@ __global__ void __launch_bounds__(256) intra_recon_kernel(kvz_cuda_quant_params 
 {
   constexpr int W = 1 << LOG2W, WW = W * W, NREF = 2 * W + 1;
   constexpr int E = 1024, G = E / WW;               // 1, 4, 16, 64 TUs per CTA
-  constexpr int PIXMAX = (1 << PixTraits<T>::kBits) - 1;
+  constexpr int PIXMAX = (1 << PixTraits<T>::bd) - 1;
   constexpr int NCG = WW / 16;                      // coefficient groups per TU
   __shared__ __align__(16) int16_t s_a[E], s_b[E], s_q[E];
   __shared__ int32_t s_d[E];
@@ -87,7 +87,7 @@ __global__ void __launch_bounds__(256) intra_recon_kernel(kvz_cuda_quant_params 
     const int gb = e / (2 * NREF), r = e - gb * 2 * NREF;
     const bool is_top = r < NREF;
     const int k = is_top ? r : r - NREF;
-    s_ref[gb][is_top ? 2 : 3][k] = (T)filter_ref_entry(s_ref[gb][0], s_ref[gb][1], is_top, k, NREF);
+    s_ref[gb][is_top ? 2 : 3][k] = (T)ref_smooth_entry(s_ref[gb][0], s_ref[gb][1], is_top, k, NREF);
   }
   for (int gb = threadIdx.x; gb < G; gb += blockDim.x) s_dc[gb] = dc_value(LOG2W, s_ref[gb][0], s_ref[gb][1]);
   __syncthreads();
@@ -101,7 +101,7 @@ __global__ void __launch_bounds__(256) intra_recon_kernel(kvz_cuda_quant_params 
       const long off = (long)((b / blocks_x) * W + y) * stride + (b % blocks_x) * W + x;
       if (INTER) pv = rec_in[off];
       else if (PHASE == 2) pv = rec_out[off];          // the forward half parked the prediction in the reconstruction plane
-      else pv = intra_predict_px(LOG2W, s_mode[gb], color, true, s_ref[gb][0], s_ref[gb][1], s_ref[gb][2], s_ref[gb][3], s_dc[gb], x, y);
+      else pv = intra_predict_px<T>(RefView<T>{ s_ref[gb][0], s_ref[gb][1], s_ref[gb][2], s_ref[gb][3], s_dc[gb] }, LOG2W, s_mode[gb], color, true, x, y);
       sv = src[off];
       if (PHASE == 1) rec_out[off] = (T)pv;
     }
@@ -158,7 +158,9 @@ __global__ void __launch_bounds__(256) intra_recon_kernel(kvz_cuda_quant_params 
       if (s_ac[gb] < 2 || !s_cgnz[gb][cg]) continue;
       const int mode = s_mode[gb];
       const int scan = ((!is_c && W <= 8) || (is_c && W == 4)) ? ((mode >= 6 && mode <= 14) ? 2 : ((mode >= 22 && mode <= 30) ? 1 : 0)) : 0;
-      sign_hide_group(s_b + gb * WW, s_q + gb * WW, s_d + gb * WW, s_cgnz[gb], NCG, cg, scan, l2);
+      int pos[16];
+      group_scan(pos, scan, l2, cg);
+      quant_sign_hiding(pos, s_b + gb * WW, s_q + gb * WW, s_d + gb * WW, s_cgnz[gb], NCG, cg);
     }
     __syncthreads();
   }
@@ -217,7 +219,7 @@ __global__ void __launch_bounds__(256) intra_recon_kernel(kvz_cuda_quant_params 
     if (first + gb < nblk) {
       if (INTER) reinterpret_cast<int32_t *>(has_out)[first + gb] = s_has[gb];
       else has_out[first + gb] = (uint8_t)s_has[gb];
-      ssd_out[first + gb] = (uint32_t)(s_ssd[gb] >> (2 * (PixTraits<T>::kBits - 8)));
+      ssd_out[first + gb] = (uint32_t)(s_ssd[gb] >> (2 * (PixTraits<T>::bd - 8)));
     }
 }
 
@@ -229,17 +231,6 @@ struct SaoPlanesT {
   int Wp[3], Hp[3];
 };
 using SaoPlanes = SaoPlanesT<uint8_t>;
-
-__device__ __forceinline__ void fp_eo_offsets(int eo, int &ax, int &ay)
-{
-  ax = (eo == 1) ? 0 : (eo == 3 ? 1 : -1);
-  ay = (eo == 0) ? 0 : -1;
-}
-__device__ __forceinline__ int fp_eo_cat(int a, int b, int c)
-{
-  const int idx = 2 + ((c > a) - (c < a)) + ((c > b) - (c < b));
-  return (0x43021 >> (4 * idx)) & 7;
-}
 
 // One CTA per (plane, CTU): ONE pass over the CTU gathers the edge statistics of all four classes
 // (calc_sao_edge_dir, ref: sao-generic.c:50-81) and the per-band sums; everything else follows in closed form:
@@ -256,7 +247,7 @@ __global__ void __launch_bounds__(256) sao_ctu_kernel(SaoPlanesT<T> pl, int nctu
                                                       int8_t *__restrict__ best, int32_t *__restrict__ dec_off,
                                                       uint32_t *__restrict__ cksum_scratch)
 {
-  constexpr int BD = PixTraits<T>::kBits;
+  constexpr int BD = PixTraits<T>::bd;
   __shared__ int s_acc[4][2][5];
   __shared__ int s_band[2][4];
   const int i = blockIdx.x, color = i / nctu, ctu = i - color * nctu;
@@ -291,8 +282,8 @@ __global__ void __launch_bounds__(256) sao_ctu_kernel(SaoPlanesT<T> pl, int nctu
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
         int ax, ay;
-        fp_eo_offsets(e, ax, ay);
-        const int cat = fp_eo_cat(rec[(long)(y + ay) * Wp + x + ax], rec[(long)(y - ay) * Wp + x - ax], c);
+        sao_eo_offsets(e, ax, ay);
+        const int cat = sao_eo_cat(rec[(long)(y + ay) * Wp + x + ax], rec[(long)(y - ay) * Wp + x - ax], c);
         cntp[e] += 1u << (6 * cat);
         const int v = diffr * ((cat & 1) ? 65536 : 1);
         sump[e][0] += cat < 2 ? v : 0;
@@ -350,22 +341,17 @@ __global__ void __launch_bounds__(256) sao_apply_kernel(SaoPlanesT<T> pl, int nc
   const T *rec = pl.rec[color];
   T *out = pl.out[color];
   const int eo = best[i];
-  int off[5];
+  EdgeOffsets off;
 #pragma unroll
-  for (int k = 0; k < 5; ++k) off[k] = dec_off[(size_t)i * 5 + k];
+  for (int k = 0; k < 5; ++k) off.o[k] = dec_off[(size_t)i * 5 + k];
   int ax = 0, ay = 0;
-  if (eo >= 0) fp_eo_offsets(eo, ax, ay);
+  if (eo >= 0) sao_eo_offsets(eo, ax, ay);
   for (int t = threadIdx.x; t < bw * bh; t += blockDim.x) {
     const int y = y0 + t / bw, x = x0 + t % bw;
     const long o = (long)y * Wp + x;
     int v = rec[o];
-    if (eo >= 0 && x >= 1 && y >= 1 && x < Wp - 1 && y < Hp - 1) {
-      const int cat = fp_eo_cat(rec[o + (long)ay * Wp + ax], rec[o - (long)ay * Wp - ax], v);
-      int ov = off[0];
-#pragma unroll
-      for (int k = 1; k < 5; ++k) ov = cat == k ? off[k] : ov;
-      v = clip3(0, (1 << PixTraits<T>::kBits) - 1, v + ov);
-    }
+    if (eo >= 0 && x >= 1 && y >= 1 && x < Wp - 1 && y < Hp - 1)
+      v = sao_edge_px(v, rec[o + (long)ay * Wp + ax], rec[o - (long)ay * Wp - ax], PixTraits<T>::bd, off);
     out[o] = (T)v;
   }
 }
@@ -715,7 +701,7 @@ size_t kvz_cuda_fp_frame_bytes(const kvz_cuda_frame_pass *fp) { return fp ? (siz
 template <class T>
 static int fp_run_dev_t(kvz_cuda_frame_pass *fp, const void *src_dev, const void *rec_in_dev, cudaStream_t st)
 {
-  constexpr int BD = PixTraits<T>::kBits;
+  constexpr int BD = PixTraits<T>::bd;
   const int W = fp->W, H = fp->H;
   const T *src = (const T *)src_dev;
   const T *rin = rec_in_dev ? (const T *)rec_in_dev : src;

@@ -26,7 +26,7 @@ __global__ void __launch_bounds__(256) intra_predict_kernel(int level, int log2w
   __syncthreads();
   for (int e = threadIdx.x; e < g * 2 * n; e += blockDim.x) {
     const int b = e / (2 * n), r = e - b * 2 * n, which = r / n, i = r - which * n;
-    s_ref[b][2 + which][i] = (T)filter_ref_entry(s_ref[b][0], s_ref[b][1], which == 0, i, n);
+    s_ref[b][2 + which][i] = (T)ref_smooth_entry(s_ref[b][0], s_ref[b][1], which == 0, i, n);
   }
   if (threadIdx.x < g) s_dc[threadIdx.x] = dc_value(log2w, s_ref[threadIdx.x][0], s_ref[threadIdx.x][1]);
   __syncthreads();
@@ -40,7 +40,7 @@ __global__ void __launch_bounds__(256) intra_predict_kernel(int level, int log2w
       else if (mode == 1) v = filtered_dc_px(top, left, s_dc[b], x, y);
       else v = angular_px(mode, top, left, x, y);
     } else {
-      v = intra_predict_px(log2w, mode, color, filter_boundary != 0, top, left, s_ref[b][2], s_ref[b][3], s_dc[b], x, y);
+      v = intra_predict_px<T>(RefView<T>{ top, left, s_ref[b][2], s_ref[b][3], s_dc[b] }, log2w, mode, color, filter_boundary != 0, x, y);
     }
     dst[(size_t)(first + b) * ww + r] = (T)v;
   }

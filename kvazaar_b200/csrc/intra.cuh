@@ -1,148 +1,19 @@
-// intra.cuh -- intra prediction device primitives.
-// Reference: src/strategies/generic/intra-generic.c (angular :49-155, planar :165-201, filtered DC :210-241) and
-// the non-dispatched wrapper logic in src/intra.c (reference smoothing :176-204, kvz_intra_predict :252-302,
-// kvz_intra_build_reference :305-559).  Every prediction sample has a closed form in the reference samples, so
-// each thread computes its own pixels directly -- no sequential accumulation, no transposition pass.
+// intra.cuh -- intra prediction device primitives of the strategy kernels.
+// The prediction rules themselves (angular, planar, DC, the edge filter, reference smoothing and availability) are
+// in pixel_rules.h, shared with the CTU search.  Every prediction sample has a closed form in the reference samples,
+// so each thread computes its own pixels directly -- no sequential accumulation, no transposition pass.  Here: the
+// reference build of kvz_intra_build_reference (ref: src/intra.c:305-559) over a frame plane.
 #pragma once
 #include "common.cuh"
 
 namespace kvzc {
 
-struct IntraRefs {          // index 0 = top-left corner sample, 1..2w = along the edge
-  const void *top, *left;   // unfiltered
-  const void *ftop, *fleft; // [1 2 1]-smoothed (only valid where the caller built them)
+// the references of one block as intra_predict_px reads them (pixel_rules.h)
+template <class T> struct RefView {
+  const T *top, *left;      // unfiltered
+  const T *ftop, *fleft;    // [1 2 1]-smoothed (only read where intra_uses_filtered)
+  int dc;                   // dc_value of the unfiltered references
 };
-
-__device__ __forceinline__ int intra_sample_disp(int mode_disp_abs)
-{
-  // sample displacement per row in 1/32 pel for |mode - 26| or |10 - mode| = 0..8
-  const int tab[9] = { 0, 2, 5, 9, 13, 17, 21, 26, 32 };
-  return tab[mode_disp_abs];
-}
-__device__ __forceinline__ int intra_inv_disp(int mode_disp_abs)
-{
-  const int tab[9] = { 0, 4096, 1638, 910, 630, 482, 390, 315, 256 };   // round(8192 / disp)
-  return tab[mode_disp_abs];
-}
-
-// Main-reference sample at block coordinate idx (>= -w .. 2w-1); negative idx < -1 project onto the side reference.
-template <class T>
-__device__ __forceinline__ int ang_ref(const T *rmain, const T *rside, int idx, int inv)
-{
-  if (idx >= -1) return rmain[idx + 1];
-  const int k = -idx - 1;
-  return rside[(128 + k * inv) >> 8];
-}
-
-// One angular sample (mode 2..34) at output position (ox, oy).
-template <class T>
-__device__ __forceinline__ int angular_px(int mode, const T *top, const T *left, int ox, int oy)
-{
-  const bool vertical = mode >= 18;
-  const int mdisp = vertical ? mode - 26 : 10 - mode;
-  const int adisp = abs(mdisp);
-  const int sdisp = mdisp < 0 ? -intra_sample_disp(adisp) : intra_sample_disp(adisp);
-  const T *rmain = vertical ? top : left;
-  const T *rside = vertical ? left : top;
-  const int x = vertical ? ox : oy, y = vertical ? oy : ox;
-  if (sdisp == 0) return rmain[x + 1];
-  const int pos = (y + 1) * sdisp;
-  const int di = pos >> 5, df = pos & 31;
-  const int inv = intra_inv_disp(adisp);
-  const int r1 = ang_ref(rmain, rside, x + di, inv);
-  if (df == 0) return r1;
-  const int r2 = ang_ref(rmain, rside, x + di + 1, inv);
-  return ((32 - df) * r1 + df * r2 + 16) >> 5;
-}
-
-template <class T>
-__device__ __forceinline__ int planar_px(int log2w, const T *top, const T *left, int x, int y)
-{
-  const int w = 1 << log2w;
-  const int hor = (w - 1 - x) * left[y + 1] + (x + 1) * top[w + 1];
-  const int ver = (w - 1 - y) * top[x + 1] + (y + 1) * left[w + 1];
-  return (ver + hor + w) >> (log2w + 1);
-}
-
-template <class T>
-__device__ __forceinline__ int dc_value(int log2w, const T *top, const T *left)
-{
-  const int w = 1 << log2w;
-  int s = 0;
-  for (int i = 1; i <= w; ++i) s += top[i] + left[i];
-  return (s + w) >> (log2w + 1);
-}
-
-template <class T>
-__device__ __forceinline__ int filtered_dc_px(const T *top, const T *left, int dc, int x, int y)
-{
-  if (x == 0 && y == 0) return (left[1] + 2 * dc + top[1] + 2) >> 2;
-  if (y == 0) return (top[x + 1] + 3 * dc + 2) >> 2;
-  if (x == 0) return (left[y + 1] + 3 * dc + 2) >> 2;
-  return dc;
-}
-
-// should kvz_intra_predict use the smoothed references?  (ref: intra.c:262-277)
-__device__ __forceinline__ bool intra_uses_filtered(int log2w, int mode, int color)
-{
-  if (color != 0 || mode == 1 || log2w == 2) return false;
-  if (mode == 0) return true;
-  const int thres = log2w == 3 ? 7 : (log2w == 4 ? 1 : 0);
-  return min(abs(mode - 26), abs(mode - 10)) > thres;
-}
-
-// kvz_intra_predict semantics for one sample.  dc = dc_value of the refs actually used (unfiltered for DC).
-template <class T>
-__device__ __forceinline__ int intra_predict_px(int log2w, int mode, int color, bool filter_boundary, const T *top,
-                                                const T *left, const T *ftop, const T *fleft, int dc, int x, int y)
-{
-  constexpr int PIXMAX = (1 << PixTraits<T>::kBits) - 1;
-  const bool f = intra_uses_filtered(log2w, mode, color);
-  const T *t = f ? ftop : top, *l = f ? fleft : left;
-  if (mode == 0) return planar_px(log2w, t, l, x, y);
-  if (mode == 1) return (color == 0 && log2w < 5) ? filtered_dc_px(t, l, dc, x, y) : dc;
-  int v = angular_px(mode, t, l, x, y);
-  if (color == 0 && log2w < 5 && filter_boundary) {           // ref: intra.c:207-219, 293-300
-    if (mode == 10 && y == 0) v = clip3(0, PIXMAX, v + ((t[x + 1] - t[0]) >> 1));
-    else if (mode == 26 && x == 0) v = clip3(0, PIXMAX, v + ((l[y + 1] - l[0]) >> 1));
-  }
-  return v;
-}
-
-// [1 2 1] smoothing of one reference entry (ref: intra.c:176-204); n = 2w+1 entries
-template <class T>
-__device__ __forceinline__ int filter_ref_entry(const T *top, const T *left, bool is_top, int i, int n)
-{
-  if (i == 0) return (left[1] + 2 * left[0] + top[1] + 2) >> 2;
-  const T *p = is_top ? top : left;
-  if (i == n - 1) return p[i];
-  return (p[i - 1] + 2 * p[i] + p[i + 1] + 2) >> 2;
-}
-
-// ---- availability (ref: intra.c:47-82): z-order rule, see oracle/kvz_oracle.c for the derivation
-__device__ __forceinline__ int zidx16(int ux, int uy)
-{
-  int z = 0;
-#pragma unroll
-  for (int b = 0; b < 4; ++b) z |= (((ux >> b) & 1) << (2 * b)) | (((uy >> b) & 1) << (2 * b + 1));
-  return z;
-}
-__device__ __forceinline__ int ref_px_top(int uy, int ux)
-{
-  if (uy == 0) return 64;
-  const int z = zidx16(ux, uy);
-  int n = 0;
-  while (ux + n < 16 && zidx16(ux + n, uy - 1) < z) ++n;
-  return 4 * n;
-}
-__device__ __forceinline__ int ref_px_left(int uy, int ux)
-{
-  if (ux == 0) return 4 * (16 - uy);
-  const int z = zidx16(ux, uy);
-  int n = 0;
-  while (uy + n < 16 && zidx16(ux - 1, uy + n) < z) ++n;
-  return 4 * n;
-}
 
 // Per-block constants of kvz_intra_build_reference over a frame plane
 struct BuildRefCtx {
@@ -158,19 +29,17 @@ __device__ __forceinline__ BuildRefCtx build_ref_ctx(int log2w, int color, int l
   c.px = luma_x >> is_c; c.py = luma_y >> is_c;
   c.has_left = luma_x > 0; c.has_top = luma_y > 0;
   c.inner = c.has_left && c.has_top;
-  int al = 0, at = 0;
-  if (c.has_left) { al = ref_px_left(ly >> 2, lx >> 2) >> is_c; al = min(al, 2 * w); al = min(al, (pic_h - luma_y) >> is_c); }
-  if (c.has_top) { at = ref_px_top(ly >> 2, lx >> 2) >> is_c; at = min(at, 2 * w); at = min(at, (pic_w - luma_x) >> is_c); }
-  // _inner copies groups of four (at least one group) before replicating (ref: intra.c:486-494, 512-516)
-  c.n_left = c.inner ? max(4, (al + 3) & ~3) : al;
-  c.n_top = c.inner ? max(4, (at + 3) & ~3) : at;
+  const int al = c.has_left ? ref_avail(ref_px_left(ly >> 2, lx >> 2), is_c, w, pic_h - luma_y) : 0;
+  const int at = c.has_top ? ref_avail(ref_px_top(ly >> 2, lx >> 2), is_c, w, pic_w - luma_x) : 0;
+  c.n_left = ref_copied(c.inner, al);
+  c.n_top = ref_copied(c.inner, at);
   return c;
 }
 // entry i (0 = corner, 1..2w) of the left / top reference
 template <class T>
 __device__ __forceinline__ int build_ref_entry(const BuildRefCtx &c, const T *rec, int stride, bool is_top, int i)
 {
-  constexpr int DC = 1 << (PixTraits<T>::kBits - 1);
+  constexpr int DC = 1 << (PixTraits<T>::bd - 1);
 #define KVZC_REC(xx, yy) ((int)rec[(long)(yy) * stride + (xx)])
   // left[1] is needed for the non-inner corner
   auto left_at = [&](int k) -> int {   // k = 0..2w-1

@@ -11,7 +11,7 @@ static __constant__ int8_t c_chroma_fir[8][4] = {
   { 0, 64, 0, 0 }, { -2, 58, 10, -2 }, { -4, 54, 16, -2 }, { -6, 46, 28, -4 },
   { -4, 36, 36, -4 }, { -4, 28, 46, -6 }, { -2, 16, 54, -4 }, { -2, 10, 58, -2 } };
 
-template <class T> __device__ __forceinline__ int clip_pix(int v) { return clip3(0, (1 << PixTraits<T>::kBits) - 1, v); }
+template <class T> __device__ __forceinline__ int clip_pix(int v) { return clip3(0, (1 << PixTraits<T>::bd) - 1, v); }
 
 // sample_quarterpel_luma(_hi) / sample_octpel_chroma(_hi) (ref: ipol-generic.c:134-211, 681-758): one CTA per block.
 // Horizontal pass into shared int16 rows, then vertical pass; intermediate truncation to int16 as in the reference.
@@ -20,7 +20,7 @@ __global__ void __launch_bounds__(256) sample_kernel(int kind, const T *__restri
                                                      void *__restrict__ dst_base, int dst_stride,
                                                      const kvz_cuda_ipol *__restrict__ descs)
 {
-  constexpr int BITS = PixTraits<T>::kBits;
+  constexpr int BITS = PixTraits<T>::bd;
   __shared__ int16_t s_h[(64 + 7) * 64];
   const kvz_cuda_ipol d = descs[blockIdx.x];
   const bool chroma = kind >= KVZ_CUDA_IPOL_CHROMA, hi = kind & 1;
@@ -55,7 +55,7 @@ __global__ void __launch_bounds__(256) sample_kernel(int kind, const T *__restri
 // Every output is  clip(((int16)(vertical_tap_sum >> 6) + 32) >> 6)  for 8-bit.
 template <class T> __device__ __forceinline__ int fme_round(int16_t s)
 {
-  constexpr int BITS = PixTraits<T>::kBits;
+  constexpr int BITS = PixTraits<T>::bd;
   const int wp_shift = 14 - BITS, wp_off = 1 << (wp_shift - 1);
   return clip_pix<T>(((int)s + wp_off) >> wp_shift);
 }
@@ -71,7 +71,7 @@ __device__ __forceinline__ int fir8_im(const int8_t *f, const int16_t *p, int st
 template <class T>
 __device__ void fme_hor(const T *src, int ss, int w, int rows, int first_y, const int8_t *f, int16_t *im_k, int16_t *col_k)
 {
-  constexpr int shift1 = PixTraits<T>::kBits - 8;
+  constexpr int shift1 = PixTraits<T>::bd - 8;
   for (int i = threadIdx.x; i < (rows - first_y) * (w + 1); i += blockDim.x) {
     const int y = first_y + i / (w + 1), x = i % (w + 1) - 1;       // x = -1 is the "first column" array
     const int v = fir8_px<T>(f, src + (long)(y - 3) * ss + (x < 0 ? -3 : x - 2), 1) >> shift1;
@@ -98,7 +98,7 @@ __global__ void __launch_bounds__(256) fme_kernel(int stage, const T *__restrict
                                                   int fme_level, int16_t *__restrict__ cols_all,
                                                   const int8_t *__restrict__ hpel_off)
 {
-  constexpr int shift1 = PixTraits<T>::kBits - 8;
+  constexpr int shift1 = PixTraits<T>::bd - 8;
   const int b = blockIdx.x;
   const T *src = src_plane + src_off[b];
   T *filtered = filtered_all + (size_t)b * 4 * 4096;

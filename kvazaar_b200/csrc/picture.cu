@@ -19,7 +19,7 @@ __global__ void __launch_bounds__(128) satd_nxn_kernel(const T *__restrict__ a, 
   constexpr int S = N / 8;
   constexpr int SUBS = S * S;
   constexpr int L = SUBS < 32 ? SUBS : 32;
-  constexpr int SHIFT = PixTraits<T>::kBits - 8;
+  constexpr int SHIFT = PixTraits<T>::bd - 8;
   const long tid = (long)blockIdx.x * blockDim.x + threadIdx.x;
   const long pair = tid / L;
   const int lane = (int)(tid % L);
@@ -87,7 +87,7 @@ __global__ void __launch_bounds__(128) sad_nxn_kernel(const T *__restrict__ a, c
 {
   constexpr int CHUNKS = N * N * (int)sizeof(T) / 16;
   constexpr int L = CHUNKS < 32 ? CHUNKS : 32;
-  constexpr int SHIFT = PixTraits<T>::kBits - 8;
+  constexpr int SHIFT = PixTraits<T>::bd - 8;
   const long tid = (long)blockIdx.x * blockDim.x + threadIdx.x;
   const long pair = tid / L;
   const int lane = (int)(tid % L);
@@ -162,7 +162,7 @@ __global__ void __launch_bounds__(128) block_cost_kernel(int op, const T *__rest
                                                          const kvz_cuda_blk *__restrict__ descs, int count,
                                                          uint32_t *__restrict__ out)
 {
-  constexpr int SHIFT = PixTraits<T>::kBits - 8;
+  constexpr int SHIFT = PixTraits<T>::bd - 8;
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (warp >= count) return;
@@ -221,7 +221,7 @@ __global__ void __launch_bounds__(128) satd_quad_kernel(const T *__restrict__ pr
                                                         const kvz_cuda_quad *__restrict__ descs, int count,
                                                         uint32_t *__restrict__ costs)
 {
-  constexpr int SHIFT = PixTraits<T>::kBits - 8;
+  constexpr int SHIFT = PixTraits<T>::bd - 8;
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (warp >= count) return;
@@ -260,7 +260,7 @@ template <class T>
 __global__ void bipred_plane_kernel(T *__restrict__ dst, int dst_stride, const void *__restrict__ l0,
                                     const void *__restrict__ l1, int im0, int im1, int w, int h)
 {
-  constexpr int BITS = PixTraits<T>::kBits;
+  constexpr int BITS = PixTraits<T>::bd;
   const int shift = 15 - BITS, offset = 1 << (shift - 1);
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= w * h) return;

@@ -29,7 +29,7 @@ namespace kvzc {
 template <class T>
 __device__ __forceinline__ uint32_t interp2(uint32_t a, uint32_t b, uint32_t f0, uint32_t f1)
 {
-  constexpr uint32_t MASK = ((1u << PixTraits<T>::kBits) - 1u) * 0x00010001u;
+  constexpr uint32_t MASK = ((1u << PixTraits<T>::bd) - 1u) * 0x00010001u;
   return ((a * f0 + b * f1 + 0x00100010u) >> 5) & MASK;           // two samples: ((32-f)*a + f*b + 16) >> 5
 }
 
@@ -48,7 +48,6 @@ __global__ void __launch_bounds__(128) rough_search_u8_kernel(const T *__restric
   constexpr int R = W >= 8 ? 8 : 4;                              // rows / cols of a lane's sub-block
   constexpr int K = R / 2;                                       // packed lane registers per row
   constexpr bool WIDE = sizeof(T) == 2;                          // 16-bit samples
-  constexpr int PIXMAX = (1 << PixTraits<T>::kBits) - 1;
   __shared__ __align__(16) T s_ref[GROUP][4][RS];                // top, left, smoothed top, smoothed left
   __shared__ __align__(16) T s_plain[GROUP][4][ES];              // same, shifted so that index j = idx + W
   __shared__ __align__(16) T s_ext[4][GROUP][ES];                // per-warp scratch: main ref with projected side part
@@ -80,7 +79,7 @@ __global__ void __launch_bounds__(128) rough_search_u8_kernel(const T *__restric
     const int gb = e / (2 * N), r = e - gb * 2 * N;
     const bool is_top = r < N;
     const int k = is_top ? r : r - N;
-    s_ref[gb][is_top ? 2 : 3][k] = (T)filter_ref_entry(s_ref[gb][0], s_ref[gb][1], is_top, k, N);
+    s_ref[gb][is_top ? 2 : 3][k] = (T)ref_smooth_entry(s_ref[gb][0], s_ref[gb][1], is_top, k, N);
   }
   if (threadIdx.x < GROUP) s_dc[threadIdx.x] = dc_value(LOG2W, s_ref[threadIdx.x][0], s_ref[threadIdx.x][1]);
   __syncthreads();
@@ -188,13 +187,13 @@ __global__ void __launch_bounds__(128) rough_search_u8_kernel(const T *__restric
       const bool vertical = m >= 18;
       const int mdisp = vertical ? m - 26 : 10 - m;
       const int adisp = abs(mdisp);
-      const int sdisp = mdisp < 0 ? -intra_sample_disp(adisp) : intra_sample_disp(adisp);
+      const int sdisp = mdisp < 0 ? -ang_disp(adisp) : ang_disp(adisp);
       const int filt = intra_uses_filtered(LOG2W, m, 0) ? 2 : 0;
       const int main_sel = (vertical ? 0 : 1) + filt, side_sel = (vertical ? 1 : 0) + filt;
       const T *ext = s_plain[g][main_sel];
       if (sdisp < 0) {
         // main reference extended to negative indices by projecting the side reference (ref: intra-generic.c:88-108)
-        const int inv = intra_inv_disp(adisp);
+        const int inv = ang_inv(adisp);
         __syncwarp();
         for (int e = lane; e < GROUP * 2 * W; e += 32) {
           const int gb = e / (2 * W), j = e - gb * 2 * W, idx = j - W;
@@ -249,8 +248,8 @@ __global__ void __launch_bounds__(128) rough_search_u8_kernel(const T *__restric
           P[0] = interp2<T>(L0, L1, f0, f1); P[1] = interp2<T>(L1, L2, f0, f1);
         }
         }
-        if (edge) {   // first column: + (side[y+1] - side[0]) >> 1, clipped (only modes 10 / 26, displacement 0)
-          const int v = clip3(0, PIXMAX, (int)(P[0] & 0xffffu) + (((int)side_unf[ey * R + r + 1] - (int)side_unf[0]) >> 1));
+        if (edge) {   // first column: the edge filter of modes 10 / 26 (displacement 0)
+          const int v = intra_edge_px<T>((int)(P[0] & 0xffffu), side_unf[ey * R + r + 1], side_unf[0]);
           P[0] = (P[0] & 0xffff0000u) | (uint32_t)v;
         }
 #pragma unroll
@@ -262,7 +261,7 @@ __global__ void __launch_bounds__(128) rough_search_u8_kernel(const T *__restric
     else cost = (hadamard4x4_lanes(d) + 1) >> 1;
 #pragma unroll
     for (int o = SUBS / 2; o > 0; o >>= 1) cost += __shfl_xor_sync(0xffffffffu, cost, o);
-    if (sub == 0) s_cost[g][m] = W >= 8 ? cost >> (PixTraits<T>::kBits - 8) : cost;   // satd_NxN shifts by the extra bit depth, satd_4x4 does not
+    if (sub == 0) s_cost[g][m] = W >= 8 ? cost >> (PixTraits<T>::bd - 8) : cost;   // satd_NxN shifts by the extra bit depth, satd_4x4 does not
   }
   __syncthreads();
   // ---- the 35 costs of every block (optional) and the fused selection: first minimum (search order of the pass)

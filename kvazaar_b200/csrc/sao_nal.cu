@@ -4,19 +4,6 @@
 
 namespace kvzc {
 
-// a/b neighbour offsets per EO class (ref: sao.h:71-76)
-__device__ __forceinline__ void eo_offsets(int eo, int &ax, int &ay, int &bx, int &by)
-{
-  ax = (eo == 1) ? 0 : (eo == 3 ? 1 : -1);  ay = (eo == 0) ? 0 : -1;
-  bx = -ax;                                  by = -ay;
-}
-// edge category (ref: sao_shared_generics.h:41-50): idx = 2 + sign(c-a) + sign(c-b) -> {1,2,0,3,4}
-__device__ __forceinline__ int eo_cat(int a, int b, int c)
-{
-  const int idx = 2 + ((c > a) - (c < a)) + ((c > b) - (c < b));
-  return (0x43021 >> (4 * idx)) & 7;
-}
-
 // calc_sao_edge_dir for all four classes of one contiguous bw x bh block pair: one CTA per block.
 template <class T>
 __global__ void __launch_bounds__(256) sao_edge_stats_kernel(int bitdepth, const T *__restrict__ orig_base,
@@ -44,9 +31,9 @@ __global__ void __launch_bounds__(256) sao_edge_stats_kernel(int bitdepth, const
     const int diff = ((int)orig[y * so + x] - c + offset) >> shift;
 #pragma unroll
     for (int e = 0; e < 4; ++e) {
-      int ax, ay, bx, by;
-      eo_offsets(e, ax, ay, bx, by);
-      const int cat = eo_cat(rec[(y + ay) * sr + x + ax], rec[(y + by) * sr + x + bx], c);
+      int ax, ay;
+      sao_eo_offsets(e, ax, ay);
+      const int cat = sao_eo_cat(rec[(y + ay) * sr + x + ax], rec[(y - ay) * sr + x - ax], c);
 #pragma unroll
       for (int k = 0; k < 5; ++k) { const int hit = cat == k; sum[e][k] += hit ? diff : 0; cnt[e][k] += hit; }
     }
@@ -74,20 +61,18 @@ __global__ void __launch_bounds__(256) sao_edge_dd_kernel(int bitdepth, const T 
   const int bw = d.bw, bh = d.bh, eo = eo_class[blockIdx.x];
   const int so = d.stride_orig ? d.stride_orig : bw, sr = d.stride_rec ? d.stride_rec : bw;
   const int bit_offset = bitdepth != 8 ? 1 << (bitdepth - 9) : 0, shift = bitdepth - 8;
-  int off[5];
+  EdgeOffsets off;
 #pragma unroll
-  for (int k = 0; k < 5; ++k) off[k] = offsets[(size_t)blockIdx.x * 5 + k];
-  int ax, ay, bx, by;
-  eo_offsets(eo, ax, ay, bx, by);
+  for (int k = 0; k < 5; ++k) off.o[k] = offsets[(size_t)blockIdx.x * 5 + k];
+  int ax, ay;
+  sao_eo_offsets(eo, ax, ay);
   int sum = 0;
   const int iw = bw - 2, ih = bh - 2;
   for (int i = threadIdx.x; i < iw * ih; i += blockDim.x) {
     const int y = 1 + i / iw, x = 1 + i % iw;
     const int c = rec[y * sr + x];
-    const int cat = eo_cat(rec[(y + ay) * sr + x + ax], rec[(y + by) * sr + x + bx], c);
-    int o = off[0];
-#pragma unroll
-    for (int k = 1; k < 5; ++k) o = cat == k ? off[k] : o;
+    const int cat = sao_eo_cat(rec[(y + ay) * sr + x + ax], rec[(y - ay) * sr + x - ax], c);
+    const int o = off[cat];
     if (o != 0) {
       const int diff = ((int)orig[y * so + x] - c + bit_offset) >> shift;
       const int delta = diff - o;
@@ -137,26 +122,19 @@ __global__ void __launch_bounds__(256) sao_reconstruct_kernel(int bitdepth, cons
                                                               T *__restrict__ new_base, int new_stride,
                                                               const kvz_cuda_sao_rec *__restrict__ descs)
 {
-  constexpr int PIXMAX_T = (1 << PixTraits<T>::kBits) - 1;
   const kvz_cuda_sao_rec d = descs[blockIdx.x];
   const T *rec = rec_base + d.off_rec;
   T *dst = new_base + d.off_new;
   const int offset_v = d.color == 2 ? 5 : 0;
-  const int values = 1 << bitdepth, shift = bitdepth - 5;
   const int bp = d.band_position[d.color == 2 ? 1 : 0];
-  int ax, ay, bx, by;
-  eo_offsets(d.eo_class, ax, ay, bx, by);
+  int ax, ay;
+  sao_eo_offsets(d.eo_class, ax, ay);
   for (int i = threadIdx.x; i < d.bw * d.bh; i += blockDim.x) {
     const int y = i / d.bw, x = i - y * d.bw;
     const T *c = rec + (long)y * stride + x;
     int v = c[0];
-    if (d.type == 1) {
-      const int k = (v >> shift) - bp;
-      if (k >= 0 && k <= 3) v = clip3(0, values - 1, v + d.offsets[k + 1 + offset_v]);
-    } else if (d.type == 2) {
-      const int cat = eo_cat(c[ay * stride + ax], c[by * stride + bx], v);
-      v = clip3(0, PIXMAX_T, v + d.offsets[cat + offset_v]);
-    }
+    if (d.type == 1) v = sao_band_px(v, bitdepth, bp, d.offsets + offset_v);
+    else if (d.type == 2) v = sao_edge_px(v, c[ay * stride + ax], c[-ay * stride - ax], PixTraits<T>::bd, d.offsets + offset_v);
     dst[(long)y * new_stride + x] = (T)v;
   }
 }

@@ -141,6 +141,13 @@ __device__ __forceinline__ int scan_pos(int scan_idx, int log2_n, int idx)
   return ((cg / gw) * 4 + (in >> 2)) * n + (cg % gw) * 4 + (in & 3);
 }
 
+// raster positions of the 16 scan positions of coefficient group g (quant_sign_hiding's scan), in registers
+__device__ __forceinline__ void group_scan(int pos[16], int scan_idx, int log2_n, int g)
+{
+#pragma unroll
+  for (int k = 0; k < 16; ++k) pos[k] = scan_pos(scan_idx, log2_n, g * 16 + k);
+}
+
 struct QuantConsts {
   int qc, q_bits, add, q_bits8;
 };
@@ -154,43 +161,6 @@ __device__ __forceinline__ QuantConsts quant_consts(const kvz_cuda_quant_params 
   c.add = (p.slice_is_intra ? 171 : 85) << (c.q_bits - 9);
   c.q_bits8 = c.q_bits - 8;
   return c;
-}
-
-// Sign-bit hiding for one 4x4 coefficient group `g` of a block (ref: quant-generic.c:84-176).  coef/q/delta_u point at
-// the block; cg_nz[h] tells whether group h had a non-zero level BEFORE any hiding.  Groups only interact through
-// "is this the last non-zero group of the scan", so one thread per group is race free.
-template <class NzT>
-__device__ __forceinline__ void sign_hide_group(const int16_t *coef, int16_t *q, const int32_t *delta_u, const NzT *cg_nz,
-                                                int num_cg, int g, int scan_idx, int log2_n)
-{
-  bool last_cg = true;
-  for (int h = g + 1; h < num_cg; ++h) if (cg_nz[h]) { last_cg = false; break; }
-  int pos[16];
-  int first_nz = 16, last_nz = -1, abssum = 0;
-#pragma unroll
-  for (int k = 0; k < 16; ++k) pos[k] = scan_pos(scan_idx, log2_n, g * 16 + k);
-  for (int k = 15; k >= 0; --k) if (q[pos[k]]) { last_nz = k; break; }
-  for (int k = 0; k < 16; ++k) if (q[pos[k]]) { first_nz = k; break; }
-  for (int k = first_nz; k <= last_nz; ++k) abssum += q[pos[k]];
-  if (last_nz - first_nz < 4) return;
-  const int signbit = q[pos[first_nz]] > 0 ? 0 : 1;
-  if (signbit == (abssum & 1)) return;
-  int min_cost = 0x7fffffff, cur_cost = 0x7fffffff, min_pos = -1;
-  int final_change = 0, cur_change = 0;
-  for (int k = (last_cg ? last_nz : 15); k >= 0; --k) {
-    const int b = pos[k];
-    if (q[b] != 0) {
-      if (delta_u[b] > 0) { cur_cost = -delta_u[b]; cur_change = 1; }
-      else if (k == first_nz && abs((int)q[b]) == 1) { cur_cost = 0x7fffffff; }
-      else { cur_cost = delta_u[b]; cur_change = -1; }
-    } else if (k < first_nz && ((coef[b] >= 0) ? 0 : 1) != signbit) {
-      cur_cost = 0x7fffffff;
-    } else { cur_cost = -delta_u[b]; cur_change = 1; }
-    if (cur_cost < min_cost) { min_cost = cur_cost; final_change = cur_change; min_pos = b; }
-  }
-  if (q[min_pos] == 32767 || q[min_pos] == -32768) final_change = -1;
-  if (coef[min_pos] >= 0) q[min_pos] = (int16_t)(q[min_pos] + final_change);
-  else q[min_pos] = (int16_t)(q[min_pos] - final_change);
 }
 
 // kvz_quant (ref: quant-generic.c:50-180) for ONE n x n block held in shared memory.
@@ -226,7 +196,9 @@ __device__ __forceinline__ void quant_block(const kvz_cuda_quant_params &p, cons
   // one thread per coefficient group: the groups only interact through "is this the last non-zero group"
   for (int g = threadIdx.x; g < num_cg; g += blockDim.x) {
     if (!s_cg_nz[g]) continue;
-    sign_hide_group(coef, q, delta_u, s_cg_nz, num_cg, g, scan_idx, log2_n);
+    int pos[16];
+    group_scan(pos, scan_idx, log2_n, g);
+    quant_sign_hiding(pos, coef, q, delta_u, s_cg_nz, num_cg, g);
   }
   __syncthreads();
 }
@@ -280,7 +252,7 @@ __device__ __forceinline__ int quantize_residual_tu(TuScratch &s, const kvz_cuda
                                                     int phase, const T *ref, int ref_stride, const T *pred,
                                                     int pred_stride, T *rec, int rec_stride, int16_t *coeff_out)
 {
-  constexpr int PIXMAX = (1 << PixTraits<T>::kBits) - 1;
+  constexpr int PIXMAX = (1 << PixTraits<T>::bd) - 1;
   const int nn = n * n, l2 = ilog2(n);
   const bool use_dst = (n == 4 && color == 0 && cu_is_intra);      // ref: strategies-dct.c:78-96
   const int ts_shift = 15 - p.bitdepth - l2;                        // ref: transform.c:150-185
